@@ -1,8 +1,8 @@
-"""B200-native sparse message-passing engine for the student-GNN distillation
+"""H100-native (sm_90a) sparse message-passing engine for the student-GNN distillation
 hot path of chaitjo/efficient-gnns (SURVEY.md §8).
 
 Layout
-  csrc/        hand-written sm_100a CUDA kernels behind the C ABI in include/b200gnn.h
+  csrc/        hand-written sm_90a CUDA kernels behind the C ABI in include/b200gnn.h
   lib.py       ctypes binding of libb200gnn.so (fails loudly if it is missing)
   ops.py       autograd-aware operators (spmm, fused BN/ReLU/dropout, losses)
   sparse.py    SparseTensor mirror (storage caches: rowptr/colptr/csr2csc/hub plan)

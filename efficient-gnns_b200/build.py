@@ -1,7 +1,7 @@
-"""In-tree build of libb200gnn.so (hand-written sm_100a CUDA behind a C ABI).
+"""In-tree build of libb200gnn.so (hand-written sm_90a CUDA for the H100, behind a C ABI).
 
-Plain ``nvcc -shared``: no torch headers, no JIT cache, so the built library
-travels with the repo snapshot to the GPU box.  Rebuilds only when a source or
+Plain ``nvcc -shared``: no torch headers, no JIT cache: the library is built
+once into the package directory and loaded from there.  Rebuilds only when a source or
 header is newer than the library.
 """
 from __future__ import annotations
@@ -39,7 +39,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     for src in sources():
         obj = obj_dir / (src.stem + ".o")
         objs.append(obj)
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                "-Xcompiler", "-fPIC", "-Xptxas=-v", "-I", str(INCLUDE), "-I", str(CSRC),
                "-c", str(src), "-o", str(obj)]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

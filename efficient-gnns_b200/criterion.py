@@ -2,7 +2,7 @@
 variant with binary cross-entropy is ``criterion_ppi.py``).
 
 Same function names, argument order and return convention ``(loss, loss_cls, loss_aux)``; every loss is computed
-by b200gnn kernels (fused row losses, edge-list passes, tcgen05 3xTF32 GEMMs for the S x S contractions) and is
+by b200gnn kernels (fused row losses, edge-list passes, wgmma 3xTF32 GEMMs for the S x S contractions) and is
 differentiable through small ``torch.autograd.Function`` wrappers.  ``from efficient_gnns_b200.criterion import *``
 in place of ``from criterion import *`` is the whole integration (INTEGRATION.md).
 
@@ -221,7 +221,7 @@ def at_criterion(logits, labels, feat, teacher_feat, beta=1000, _cls=None):
 # ----------------------------------------------------------------------------------------- GSP
 class _GSP(torch.autograd.Function):
     """mse(pairwise_k(fs), pairwise_k(ft)) over an S-row sample (criterion.py:66-86), S x S never leaves HBM twice:
-    Gram matrices by tcgen05 GEMM, similarity + MSE + d/dGram in one pass per side."""
+    Gram matrices by wgmma GEMM, similarity + MSE + d/dGram in one pass per side."""
 
     @staticmethod
     def forward(ctx, fs, ft, kernel: int):
@@ -391,13 +391,17 @@ def lpw_criterion(logits, labels, feat, teacher_feat, edge_index, kernel='cosine
 
 
 # ----------------------------------------------------------------------------------------- G-CRD
-NCE_CHUNK_BYTES = 32 << 20      # logits chunk [R, S] (+ its transpose) sized to stay L2-resident between the three GEMMs
+# Logits chunk [R, S] of the G-CRD loss.  What sets the size is how many rows R the chunk's three GEMMs get, not L2
+# residency (at 32 MB the chunk and its transpose exceed the 50 MB L2 of an H100): at S = 16384, F = 256 one forward +
+# backward takes 75 / 42 / 22 / 14 ms with 8 / 16 / 32 / 64 MB chunks (tools/bench_nce_chunk.py, H100).  32 MB keeps the
+# loss's peak memory well under that of the S x S logits it avoids (tests/test_criterion_gpu.py bounds it at S = 8192).
+NCE_CHUNK_BYTES = 32 << 20
 
 
 class _NCE(torch.autograd.Function):
     """InfoNCE between normalised student rows and teacher rows (criterion.py:139-146) WITHOUT the S x S logits tensor
     (1 GiB at the scripts' S = 16384, arxiv_pyg/scripts/run_gcn.sh:144).  The rows are streamed in chunks of R (R*S*4 <=
-    32 MB, so a chunk and its transpose live in the 126 MB L2): per chunk one [R,S] logits GEMM on the tensor cores, the
+    NCE_CHUNK_BYTES): per chunk one [R,S] logits GEMM on the tensor cores, the
     fused row pass (log-sum-exp, loss term, d/dlogits in place), and the two gradient contractions
     d fs[chunk] = dZ_c · x_t and d f_t += dZ_c^T · x_s[chunk] (accumulating epilogue) — the gradients are complete when
     the forward returns, so the backward only scales them."""

@@ -1,4 +1,4 @@
-// Shared helpers for the b200gnn kernels (sm_100a only).
+// Shared helpers for the b200gnn kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

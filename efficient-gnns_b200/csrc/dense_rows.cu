@@ -1,7 +1,7 @@
 // Row-major [n_rows, K] fp32 passes that sit between the aggregations of a student GNN layer
 // (arxiv_pyg/gnn.py:46-50: conv -> BatchNorm1d -> ReLU -> dropout) and their backward.
 // All are HBM-bound streaming kernels: 128-bit accesses, per-CTA deterministic partial
-// reductions (no atomics), grid sized to a multiple of the 148 SMs.
+// reductions (no atomics), grid sized to a multiple of the 132 SMs of an H100.
 #include "common.cuh"
 #include "philox.cuh"
 
@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
 }
 __global__ void adam_tick_kernel(int32_t* step) { *step += 1; }
 
-static inline int grid_for(int64_t n_items, int per_cta, int cap = 148 * 8) {
+static inline int grid_for(int64_t n_items, int per_cta, int cap = 132 * 8) {
   int64_t g = (n_items + per_cta - 1) / per_cta;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -411,7 +411,7 @@ static bool rows_ok(int64_t n_rows, int64_t K) { return n_rows >= 0 && K > 0 && 
 extern "C" int64_t b200gnn_rows_slots(int64_t n_rows) {
   // one slot per CTA; ~2 CTAs per SM keeps the partial buffer small and the reduction order fixed
   int64_t s = (n_rows + 255) / 256;
-  if (s > 148 * 4) s = 148 * 4;
+  if (s > 132 * 4) s = 132 * 4;
   return s < 1 ? 1 : s;
 }
 

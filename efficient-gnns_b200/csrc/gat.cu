@@ -498,7 +498,7 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_bwd_hub_finalize_kernel(const
 
 static inline int rows_grid(int64_t n) {
   int64_t g = (n + GAT_WARPS - 1) / GAT_WARPS;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   return (int)(g < 1 ? 1 : g);
 }
 

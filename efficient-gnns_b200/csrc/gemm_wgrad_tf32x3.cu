@@ -1,18 +1,18 @@
-// Weight-gradient GEMM on tcgen05:   dW[Kin, Nout] = X[Nn, Kin]^T · G[Nn, Nout]      (fp32-faithful, 3xTF32)
+// Weight-gradient GEMM on the Hopper tensor cores:   dW[Kin, Nout] = X[Nn, Kin]^T · G[Nn, Nout]   (fp32-faithful, 3xTF32)
 //
 // The contraction runs over the NODE index (Nn ~ 1.7e5) and the result is tiny (<= 256 x 256), so this is a
-// split-K problem: every CTA owns a contiguous range of nodes, streams its slice of X and G through shared memory
-// exactly once, accumulates a full Kin x Nout partial in TMEM (2 x 128 lanes x 256 columns = all 512 columns), and
-// a small second kernel adds the per-CTA partials in a fixed order (deterministic, no atomics).
+// split-K problem: the output is cut into 128 x 128 tiles, every CTA owns one tile and a contiguous range of nodes,
+// streams its slices of X and G through shared memory exactly once, keeps the tile's partial in registers, and a small
+// second kernel adds the per-range partials in a fixed order (deterministic, no atomics).
 //
-// Both operands are "MN-major" for the tensor core (the contraction index is the slow one in memory):
-//   * per 32-column group one 2-D TMA box {32 floats, 16 nodes} with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; the
-//     boxes land back to back as [group][node][32 floats], which is UMMA's canonical MN-major layout for 32-bit
-//     operands, SWIZZLE_128B_BASE32B (the only MN-major layout tf32 accepts: 32-byte chunks XOR-ed with node%4;
-//     leading byte offset = 2048 B between 32-column groups, stride byte offset = 512 B between 4-node atoms;
-//     semantics pinned with tools/umma_probe.cu);
-//   * both X and G are big activations, so both are split into tf32 hi/lo in shared memory by 4 splitter warps.
-// Warp roles as in gemm_tf32x3.cu: TMA producer, MMA issuer, TMEM allocator, 4 splitter warps, 4 epilogue warps.
+// Both operands are "MN-major" (the contraction index is the slow one in memory), and wgmma takes tf32 operands
+// K-major only.  So the consumers transpose as they split: TMA lands [32 nodes][128 columns] of X and of G, and the
+// 256 consumer threads write (hi, lo) of each as [128 rows][32 nodes] K-major tiles with the 128-byte swizzle, the
+// layout of gemm_tf32x3.cu.  The transposed tiles are double-buffered, so the split of node block i overlaps the
+// wgmmas of block i-1.  Accumulation as in gemm_tf32x3.cu: each block's 12 wgmmas go to a fresh register accumulator
+// that is added (fp32, round to nearest) into the running partial.
+//
+// 384 threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the tile each.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -20,197 +20,132 @@ namespace b200gnn {
 namespace wgrad {
 using namespace tc;
 
-constexpr int BKN = 16;                       // nodes per pipeline stage (two K=8 MMA steps)
-constexpr int MAX_STAGES = 8;
+constexpr int BKN = 32;                       // nodes per stage: one 128-byte K-major row of the transposed operands
+constexpr int TM = 128, TN = 128;             // output tile (rows of dW = columns of X, columns of dW = columns of G)
 constexpr int THREADS = 384;
-constexpr int GROUP_BYTES = BKN * 128;        // 2 KB: one 32-column group of one operand, 16 nodes x 128 B
-// A stage holds X_hi, X_lo ([Kin/32] groups each) and G_hi, G_lo ([Npad/32] groups each) back to back; the pool is cut into
-// as many stages as fit (3 at 256x256 = 64 KB per stage, 4 at 128x256, 5 at 256x64): the narrow shapes are bound by the
-// latency of the TMA -> split -> MMA -> free chain per stage, which only depth hides.
-constexpr int POOL_BYTES = 5 * 40 * 1024;
-constexpr int SMEM_BYTES = POOL_BYTES + 256 + 1024;
-constexpr int TMEM_COLS = 512;
-// The tensor core rounds its fp32 accumulator towards zero on every accumulate (tools/probe_accum.py): a CTA that
-// chains its whole node range (~430 MMAs at ARXIV size) ends 1.3e-5 low; the loss depends on HOW OFTEN the large
-// accumulator is updated, not on what is added.  Two remedies, by TMEM budget:
-//   * the partial needs <= 256 columns (Kin = 128, or Nout <= 128): the two 2^-11-sized correction terms accumulate in
-//     their own TMEM region, which takes two of every three updates off the large accumulator; the epilogue adds the pair;
-//   * Kin = 256 with Nout > 128 fills all 512 columns: the chain is cut every DRAIN_KB node blocks instead — the epilogue
-//     adds the drained partial into the CTA's workspace slot with a rounded fp32 add and the next sub-range starts from
-//     a fresh accumulator (costs a pipeline bubble per drain, ~10 us; measured error 8.1e-6 -> 1.6e-6 at 16 blocks).
-constexpr int DRAIN_KB = 24;
-
-// MN-major tile [group][node][32 floats], 128B swizzle with 32-byte atoms
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((BKN * 128) >> 4) << 16;    // leading byte offset: next 32-column group (2048 B)
-  d |= (uint64_t)(512 >> 4) << 32;            // stride byte offset: next 4-node atom (512 B)
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;                     // SWIZZLE_128B_BASE32B
-  return d;
-}
+constexpr int STAGES = 3;
+constexpr int RAW_BYTES = BKN * (TM + TN) * 4;   // 32 KB: X and G blocks as TMA lands them, [node][column]
+constexpr int OP_BYTES = 128 * BKN * 4;          // 16 KB: one transposed operand, [128 rows][32 nodes]
+constexpr int T_BYTES = 4 * OP_BYTES;            // X_hi, X_lo, G_hi, G_lo
+constexpr int SMEM_BYTES = STAGES * RAW_BYTES + 2 * T_BYTES + 256 + 1024;
+constexpr int MAX_RANGES = 132;                  // node ranges (workspace partials): one CTA per SM over all tiles
+static_assert(SMEM_BYTES <= 232448, "shared memory");
 
 struct Params {
-  float* partial;   // [grid][Kin][Npad],  Npad = Nout rounded up to 32 (TMA zero-fills the missing columns)
+  float* partial;   // [n_ranges][Kin][Npad],  Npad = Nout rounded up to 32 (TMA zero-fills the missing columns)
   int32_t Nn, Kin, Nout, Npad, num_kb;
-  int32_t mode;     // 0 automatic; A/B knobs (b200gnn_wgrad_set_mode): 1 = drains only, 2 = one chain (round-1 behaviour)
+  int32_t n_tn, n_ranges;   // column tiles of dW, node ranges
 };
 
 __global__ void __launch_bounds__(THREADS, 1)
 wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG, const Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + POOL_BYTES);
-  uint64_t* full = bars;
-  uint64_t* split = bars + MAX_STAGES;
-  uint64_t* empty = bars + 2 * MAX_STAGES;
-  uint64_t* acc_full = bars + 3 * MAX_STAGES;
-  uint64_t* acc_empty = acc_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 1);
-  const int xg = p.Kin / 32, gg = p.Npad / 32;               // 32-column groups of X and G
-  const int X_BYTES = xg * GROUP_BYTES, G_BYTES = gg * GROUP_BYTES;
-  const int STAGE_BYTES = 2 * (X_BYTES + G_BYTES);
-  const int STAGES = min(MAX_STAGES, POOL_BYTES / STAGE_BYTES);
+  uint8_t* tbuf = smem + STAGES * RAW_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(tbuf + 2 * T_BYTES);
+  uint64_t* empty = full + STAGES;
+
+  const int tiles = (p.Kin / TM) * p.n_tn;
+  const int tile = (int)blockIdx.x % tiles, range = (int)blockIdx.x / tiles;
+  const int mt = tile / p.n_tn, nt = tile % p.n_tn;
+  const int kb0 = (int)((int64_t)p.num_kb * range / p.n_ranges);
+  const int kb1 = (int)((int64_t)p.num_kb * (range + 1) / p.n_ranges);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 128);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // this CTA's node blocks
-  const int kb0 = (int)((int64_t)p.num_kb * blockIdx.x / gridDim.x);
-  const int kb1 = (int)((int64_t)p.num_kb * (blockIdx.x + 1) / gridDim.x);
-  const int mtiles = p.Kin / 128;
-  const int len = kb1 - kb0;
-  const bool sep = p.mode == 0 && ((mtiles == 1) || (p.Npad <= 128));   // room for a separate correction accumulator
-  const uint32_t corr_off = mtiles == 1 ? 256u : 128u;
-  int nd = (sep || p.mode == 2) ? 1 : (len + DRAIN_KB - 1) / DRAIN_KB;  // accumulator drains of this CTA (>= 1 when it has work)
-  if (nd < 1) nd = 1;
-  if (nd > len && len > 0) nd = len;
-  const uint32_t tx_bytes = (uint32_t)(X_BYTES + G_BYTES);
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dec<40>();
+    if (threadIdx.x == 0) {
       int s = 0; uint32_t ph = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* st = smem + s * STAGE_BYTES;
-        mbar_expect_tx(&full[s], tx_bytes);
-        for (int g = 0; g < xg; ++g) tma_load_2d(&tmX, &full[s], st + g * GROUP_BYTES, g * 32, kb * BKN);
-        for (int g = 0; g < gg; ++g) tma_load_2d(&tmG, &full[s], st + 2 * X_BYTES + g * GROUP_BYTES, g * 32, kb * BKN);
+        uint8_t* st = smem + s * RAW_BYTES;
+        mbar_expect_tx(&full[s], RAW_BYTES);
+        tma_load_2d(&tmX, &full[s], st, mt * TM, kb * BKN);
+        tma_load_2d(&tmG, &full[s], st + BKN * TM * 4, nt * TN, kb * BKN);
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // D = f32, A = B = tf32, both MN-major, M = 128, N = Nout
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |
-                             ((uint32_t)(p.Npad >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int s = 0; uint32_t ph = 0;
-      for (int d = 0; d < nd; ++d) {
-        const int d0 = kb0 + (int)((int64_t)len * d / nd), d1 = kb0 + (int)((int64_t)len * (d + 1) / nd);
-        if (d > 0) { mbar_wait(acc_empty, (uint32_t)((d - 1) & 1)); tc_fence_after(); }   // previous partial drained
-        for (int kb = d0; kb < d1; ++kb) {
-          mbar_wait(&full[s], ph);
-          mbar_wait(&split[s], ph);
-          tc_fence_after();
-          const uint32_t st = smem_u32(smem + s * STAGE_BYTES);
-#pragma unroll
-          for (int kg = 0; kg < BKN / 8; ++kg) {
-            const uint64_t g_hi = make_desc_mn(st + 2 * X_BYTES + kg * 1024);
-            const uint64_t g_lo = make_desc_mn(st + 2 * X_BYTES + G_BYTES + kg * 1024);
-            for (int mt = 0; mt < mtiles; ++mt) {
-              const uint32_t xoff = (uint32_t)(mt * 4 * BKN * 128 + kg * 1024);
-              const uint64_t x_hi = make_desc_mn(st + xoff), x_lo = make_desc_mn(st + X_BYTES + xoff);
-              const uint32_t dt = tmem_base + (uint32_t)(mt * 256);
-              const uint32_t first = (kb != d0) | (kg != 0);
-              if (sep) {
-                mma_tf32(dt + corr_off, x_lo, g_hi, idesc, first);
-                mma_tf32(dt + corr_off, x_hi, g_lo, idesc, 1);
-                mma_tf32(dt, x_hi, g_hi, idesc, first);
-              } else {
-                mma_tf32(dt, x_lo, g_hi, idesc, first);
-                mma_tf32(dt, x_hi, g_lo, idesc, 1);
-                mma_tf32(dt, x_hi, g_hi, idesc, 1);
-              }
-            }
-          }
-          mma_commit(&empty[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        mma_commit(acc_full);
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    const int t = threadIdx.x - 128;
-    const int nx = xg * BKN * 128 / 16, ng = gg * BKN * 128 / 16;   // uint4 counts
-    int s = 0; uint32_t ph = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full[s], ph);
-      uint4* xh = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES);
-      uint4* xl = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + X_BYTES);
-      uint4* gh = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + 2 * X_BYTES);
-      uint4* gl = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + 2 * X_BYTES + G_BYTES);
-      for (int o = t; o < nx; o += 128) { const uint4 v = xh[o]; uint4 h, l; split4(v, h, l); xh[o] = h; xl[o] = l; }
-      for (int o = t; o < ng; o += 128) { const uint4 v = gh[o]; uint4 h, l; split4(v, h, l); gh[o] = h; gl[o] = l; }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(&split[s]);
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-  } else if (warp >= 8) {
-    const int q = warp & 3;
-    float* out = p.partial + (size_t)blockIdx.x * p.Kin * p.Npad;
-    for (int d = 0; d < (len > 0 ? nd : 0); ++d) {
-      mbar_wait(acc_full, (uint32_t)(d & 1));
-      tc_fence_after();
-      for (int mt = 0; mt < mtiles; ++mt) {
-        const int row = mt * 128 + q * 32 + lane;
-#pragma unroll 1
-        for (int c = 0; c < gg; ++c) {
-          uint32_t r[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * 256 + c * 32), r);
-          if (sep) {
-            uint32_t rc[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * 256 + c * 32) + corr_off, rc);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(rc[j]));
-          }
-          float4* dst = reinterpret_cast<float4*>(out + (size_t)row * p.Npad + c * 32);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                                   __uint_as_float(r[4 * j + 3]));
-            if (d > 0)      // later drains ADD to the slot (same thread, same address: ordered); no read-back latency
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                           : "memory");
-            else
-              dst[j] = v;
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(acc_empty);
-    }
+    return;
   }
+  regs_inc<232>();
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
+  const int cw = (warp >> 2) - 1;             // warpgroup: rows [64 cw, 64 cw + 64) of the tile
+  const int ct = threadIdx.x - 128;           // 0..255
+  float acc[64], sum[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+  int s = 0; uint32_t ph = 0;
+  for (int kb = kb0, i = 0; kb < kb1; ++kb, ++i) {
+    mbar_wait(&full[s], ph);
+    const float* rx = reinterpret_cast<const float*>(smem + s * RAW_BYTES);   // [32 nodes][128]
+    const float* rg = rx + BKN * TM;
+    uint8_t* T = tbuf + (i & 1) * T_BYTES;
+    // transpose + split: item = (operand, row r, 4-node chunk c); consecutive threads take consecutive rows, so the
+    // reads are conflict-free and the 16-byte swizzled writes of 8 consecutive rows cover all banks
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int idx = u * 256 + ct;
+      const int op = idx >> 10, r = idx & 127, c = (idx >> 7) & 7;
+      const float* src = (op ? rg : rx) + (4 * c) * 128 + r;
+      const uint4 v = make_uint4(__float_as_uint(src[0]), __float_as_uint(src[128]), __float_as_uint(src[256]),
+                                 __float_as_uint(src[384]));
+      uint4 h, l;
+      split4(v, h, l);
+      uint8_t* base = T + op * 2 * OP_BYTES;
+      *reinterpret_cast<uint4*>(base + swz128(r, c)) = h;
+      *reinterpret_cast<uint4*>(base + OP_BYTES + swz128(r, c)) = l;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    mbar_arrive(&empty[s]);                    // the raw block has been read
+    if (i > 0) {                               // block i-1's wgmmas have retired: promote
+      wgmma_wait<0>();
+      acc_fence(acc);
+#pragma unroll
+      for (int j = 0; j < 64; ++j) sum[j] += acc[j];
+    }
+    named_sync(1, 256);                        // T[i & 1] complete; every warpgroup is done with T[(i + 1) & 1]
+    wgmma_fence();
+    const uint32_t sa = smem_u32(T);
+#pragma unroll
+    for (int k = 0; k < BKN / 8; ++k) {        // the small correction terms first (see gemm_tf32x3.cu)
+      const uint32_t koff = k * 32;
+      const uint64_t x_hi = make_desc_k128(sa + cw * (OP_BYTES / 2) + koff);
+      const uint64_t x_lo = make_desc_k128(sa + OP_BYTES + cw * (OP_BYTES / 2) + koff);
+      const uint64_t g_hi = make_desc_k128(sa + 2 * OP_BYTES + koff);
+      const uint64_t g_lo = make_desc_k128(sa + 3 * OP_BYTES + koff);
+      wgmma_tf32_n128(acc, x_lo, g_hi, k != 0);
+      wgmma_tf32_n128(acc, x_hi, g_lo, 1);
+    }
+#pragma unroll
+    for (int k = 0; k < BKN / 8; ++k) {
+      const uint32_t koff = k * 32;
+      wgmma_tf32_n128(acc, make_desc_k128(sa + cw * (OP_BYTES / 2) + koff), make_desc_k128(sa + 2 * OP_BYTES + koff), 1);
+    }
+    wgmma_commit();
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+  if (kb1 > kb0) {
+    wgmma_wait<0>();
+    acc_fence(acc);
+#pragma unroll
+    for (int j = 0; j < 64; ++j) sum[j] += acc[j];
+  }
+  // fragment -> partial: rows mt*128 + 64 cw + 16 (warp % 4) + lane/4 (+8), columns nt*128 + 8 j + 2 (lane % 4)
+  float* out = p.partial + (size_t)range * p.Kin * p.Npad;
+  const int row0 = mt * TM + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = nt * TN + 8 * j + 2 * (lane & 3);
+    if (col < p.Npad) {
+      *reinterpret_cast<float2*>(out + (size_t)row0 * p.Npad + col) = make_float2(sum[4 * j], sum[4 * j + 1]);
+      *reinterpret_cast<float2*>(out + (size_t)(row0 + 8) * p.Npad + col) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
+    }
   }
 }
 
@@ -244,16 +179,16 @@ __global__ void __launch_bounds__(RED_VECS * RED_GROUPS) wgrad_reduce_kernel(con
   *reinterpret_cast<float4*>(out + (size_t)row * Nout + c4) = acc;   // Nout % 4 == 0
 }
 
-// [rows, width] fp32 row-major (ld): boxes of 32 columns x 16 rows, 128B swizzle, zero fill past the last row
-static bool make_map_mn(CUtensorMap* m, const float* base, int64_t rows, int64_t width, int64_t ld) {
+// [rows, width] fp32 row-major (ld): boxes of 128 columns x BKN rows, no swizzle, zero fill past the last row / column
+static bool make_map_rows(CUtensorMap* m, const float* base, int64_t rows, int64_t width, int64_t ld) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return false;
   cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {32, (cuuint32_t)BKN};
+  cuuint32_t box[2] = {128, (cuuint32_t)BKN};
   cuuint32_t estr[2] = {1, 1};
   return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -262,12 +197,9 @@ static bool make_map_mn(CUtensorMap* m, const float* base, int64_t rows, int64_t
 
 using namespace b200gnn;
 
-static int g_wgrad_mode = 0;
-extern "C" void b200gnn_wgrad_set_mode(int mode) { g_wgrad_mode = mode; }
-
 extern "C" int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout) {
   if (Kin <= 0 || Nout <= 0) return B200GNN_ERR_BAD_ARG;
-  return 148 * Kin * ((Nout + 31) / 32 * 32);
+  return wgrad::MAX_RANGES * Kin * ((Nout + 31) / 32 * 32);
 }
 
 extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW,
@@ -279,32 +211,34 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const 
       !aligned_to(dW, 16) || !aligned_to(workspace, 16))
     return B200GNN_ERR_UNSUPPORTED;
   CUtensorMap tX, tG;
-  if (!wgrad::make_map_mn(&tX, X, Nn, Kin, ldx) || !wgrad::make_map_mn(&tG, G, Nn, Nout, ldg)) return B200GNN_ERR_UNSUPPORTED;
-  int dev_a = 0;
-  cudaGetDevice(&dev_a);
+  if (!wgrad::make_map_rows(&tX, X, Nn, Kin, ldx) || !wgrad::make_map_rows(&tG, G, Nn, Nout, ldg)) return B200GNN_ERR_UNSUPPORTED;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device
-  if (dev_a >= 0 && dev_a < 64 && !attr_set[dev_a]) {
+  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
     cudaError_t e = cudaFuncSetAttribute(wgrad::wgrad_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          wgrad::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
-    attr_set[dev_a] = true;
+    attr_set[dev] = true;
   }
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaStream_t st = (cudaStream_t)stream;
   wgrad::Params p;
   p.partial = workspace; p.Nn = (int32_t)Nn; p.Kin = (int32_t)Kin; p.Nout = (int32_t)Nout;
   p.Npad = (int32_t)((Nout + 31) / 32 * 32);
   p.num_kb = (int32_t)((Nn + wgrad::BKN - 1) / wgrad::BKN);
-  p.mode = g_wgrad_mode;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms > 148) sms = 148;  // workspace is sized for 148 partials
-  const int grid = p.num_kb < sms ? p.num_kb : sms;
+  p.n_tn = (p.Npad + wgrad::TN - 1) / wgrad::TN;
+  const int tiles = (int)(Kin / wgrad::TM) * p.n_tn;
+  int ranges = sms / tiles;                          // one CTA per SM over all tiles
+  if (ranges > wgrad::MAX_RANGES) ranges = wgrad::MAX_RANGES;   // the workspace holds MAX_RANGES partials
+  if (ranges > p.num_kb) ranges = p.num_kb;
+  if (ranges < 1) ranges = 1;
+  p.n_ranges = ranges;
   int rc;
-  wgrad::wgrad_tf32x3_kernel<<<grid, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
+  wgrad::wgrad_tf32x3_kernel<<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
   if ((rc = check_launch())) return rc;
   const int64_t n_vec = Kin * (int64_t)p.Npad / 4;
-  wgrad::wgrad_reduce_kernel<<<(int)((n_vec + wgrad::RED_VECS - 1) / wgrad::RED_VECS), wgrad::RED_VECS * wgrad::RED_GROUPS, 0, st>>>(reinterpret_cast<const float4*>(workspace), grid,
-                                                                        (int)Kin, (int)Nout, p.Npad, dW);
+  wgrad::wgrad_reduce_kernel<<<(int)((n_vec + wgrad::RED_VECS - 1) / wgrad::RED_VECS), wgrad::RED_VECS * wgrad::RED_GROUPS, 0, st>>>(
+      reinterpret_cast<const float4*>(workspace), ranges, (int)Kin, (int)Nout, p.Npad, dW);
   return check_launch();
 }

@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(256) rowptr_kernel(const int64_t* __restrict__
   }
 }
 
-static inline int grid1d(int64_t n, int per = 256, int cap = 148 * 16) {
+static inline int grid1d(int64_t n, int per = 256, int cap = 132 * 16) {
   int64_t g = (n + per - 1) / per;
   if (g > cap) g = cap;
   return (int)(g < 1 ? 1 : g);

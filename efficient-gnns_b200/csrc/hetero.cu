@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) typed_scatter_kernel(const float* __restr
 
 static inline int rows_grid(int64_t n) {
   int64_t g = (n + 7) / 8;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   return (int)(g < 1 ? 1 : g);
 }
 

@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(256) lsp_diag_kernel(const int32_t* __restrict
 
 static inline int edge_grid(int64_t items) {
   int64_t g = (items + 7) / 8;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   return (int)(g < 1 ? 1 : g);
 }
 

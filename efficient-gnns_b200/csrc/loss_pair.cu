@@ -1,5 +1,5 @@
 // Building blocks of the feature-distillation criteria of arxiv_pyg/criterion.py (fitnet :24-36, AT :39-54,
-// GSP/gpw :57-92, G-CRD/nce :129-149).  The S x S contractions themselves run on the tcgen05 GEMM
+// GSP/gpw :57-92, G-CRD/nce :129-149).  The S x S contractions themselves run on the wgmma GEMM
 // (gemm_tf32x3.cu); the kernels here are the row / element passes around them, each producing the forward value
 // and the tensor the backward GEMM needs in the same pass.  Loss scalars are reduced deterministically
 // (per-CTA partials, fixed-order finalize).
@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(256) bce_logits_kernel(const float* __restrict
 
 static inline int ew_grid(int64_t n, int per = 256 * 4) {
   int64_t g = (n + per - 1) / per;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   return (int)(g < 1 ? 1 : g);
 }
 

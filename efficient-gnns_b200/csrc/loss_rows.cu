@@ -116,7 +116,7 @@ using namespace b200gnn;
 
 extern "C" int64_t b200gnn_kd_partials(int64_t n_train) {
   int64_t g = (n_train + LOSS_WARPS - 1) / LOSS_WARPS;
-  if (g > 148 * 16) g = 148 * 16;   // rows are a chain of dependent loads (idx -> label -> rows): many short warps
+  if (g > 132 * 16) g = 132 * 16;   // rows are a chain of dependent loads (idx -> label -> rows): many short warps
   return g < 1 ? 1 : g;
 }
 

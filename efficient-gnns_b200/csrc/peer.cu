@@ -1,7 +1,7 @@
 // Peer-memory data path of the node-parallel engine (SURVEY.md §8e): one process per GPU, every rank maps the other
 // ranks' exchange arenas through CUDA IPC and the exchange steps of a training step are plain kernels that STORE
 // straight into the consumers' buffers over NVLink/NVSwitch, followed by a flag barrier — no collective library call on
-// the data path.  The reference is single-GPU (arxiv_pyg/scripts/run_gcn.sh:24-28); this is the B200-native extension
+// the data path.  The reference is single-GPU (arxiv_pyg/scripts/run_gcn.sh:24-28); this is the native multi-GPU extension
 // BASELINE.json's north_star asks for.
 //
 //   b200gnn_arena_alloc / _free        cudaMalloc'd arena (IPC handles need a cudaMalloc allocation, not a sub-block of
@@ -164,7 +164,7 @@ static int fill_copies(peer::CopyParams& p, const b200gnn_copy2d* copies, int32_
   if (m == 0) { *grid = dim3(0, 0); return B200GNN_OK; }
   const int64_t vecs = max_rows * p.nvec;
   int64_t per = (vecs + 1023) / 1024;                 // 256 threads x 4 float4 per pass
-  const int64_t cap = (148 * 8 + m - 1) / m;         // about 8 CTAs per SM over all copies
+  const int64_t cap = (132 * 8 + m - 1) / m;         // about 8 CTAs per SM over all copies
   if (per > cap) per = cap;
   if (per < 1) per = 1;
   *grid = dim3((unsigned)per, (unsigned)m);

@@ -1,4 +1,4 @@
-// Row-segmented CSR SpMM for sm_100a:  Y[i,:] = reduce_e val[e] * X[col[e],:]
+// Row-segmented CSR SpMM for sm_90a:  Y[i,:] = reduce_e val[e] * X[col[e],:]
 //
 // Replaces torch_sparse spmm_sum/spmm_mean as reached from the reference's
 // GCNConv / SAGEConv / SparseTensor.matmul call sites (arxiv_pyg/gnn.py:47,52,
@@ -482,13 +482,13 @@ __global__ void __launch_bounds__(SPMM_THREADS, 3) spmm_rows_pipe_kernel(const S
 
 
 // ------------------------------------------------------------------ bulk-copy (TMA) chunk kernel, column-slab tiled
-// Blackwell data path for wide rows (K a multiple of 128 floats).  Same chunk / run / row-boundary ownership as the
+// TMA bulk-copy data path for wide rows (K a multiple of 128 floats).  Same chunk / run / row-boundary ownership as the
 // cp.async kernel above, but every neighbour row (slab) is ONE cp.async.bulk (SASS UBLKCP) of 512*CH bytes issued by the
 // lane that holds its column index, completing on an mbarrier per group of G ring slots: no per-lane copy instructions,
 // no address arithmetic on 32 lanes, and the ring keeps BULK_RING bytes per warp in flight across row boundaries.
 // K is tiled into column slabs of 128*CH floats and the grid is slab-major (all chunks of slab 0, then slab 1, ...), so
-// the [N, slab] operand the resident CTAs gather from is 1/n_slabs of X and stays L2-resident (ARXIV-shape K=256: 87 MB
-// per slab against a 126 MB L2, instead of 173 MB that does not fit); (col,val) are re-read per slab (8 B per edge).
+// the [N, slab] operand the resident CTAs gather from is 1/n_slabs of X, which keeps more of it L2-resident (ARXIV-shape
+// K=256: 87 MB per 128-float slab instead of 173 MB, against a 50 MB L2); (col,val) are re-read per slab (8 B per edge).
 constexpr int BULK_RING = 8192;                  // ring bytes per warp
 constexpr int BULK_MAX_GROUPS = 8;
 
@@ -520,21 +520,9 @@ __device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32
                : "memory");
 }
 
-// TMA tile::gather4 (SASS UTMALDG.2D.GATHER4): FOUR rows of the [n_src, K] operand, `box` columns each starting at column x,
-// land back to back in shared memory for ONE instruction (tensor map with a {128 floats, 1 row} box).  The copy engine retires
-// a fixed number of instructions per second (tools/bulk_probe.cu, tools/gather4_probe.cu: ~20 G single-row copies/s, but
-// 30 G ROWS/s as 512-byte gather4 quads = 16 TB/s from an L2-resident slab), which is what makes 128-float column slabs pay.
-__device__ __forceinline__ void tma_gather4(void* dst, const CUtensorMap* tm, int x, int r0, int r1, int r2, int r3, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-      ::"r"(smem_u32(dst)), "l"(tm), "r"(x), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(smem_u32(bar))
-      : "memory");
-}
-
-template <int CH, int G, bool HAS_VAL, bool STATS, bool G4 = false>
+template <int CH, int G, bool HAS_VAL, bool STATS>
 __device__ __forceinline__ void spmm_chunk_cta_bulk(const SpmmParams& p, const int cta, const int slab, float* s_stat,
-                                                    float4* ring_all, uint64_t* bars_all, const CUtensorMap* tm = nullptr) {
-  static_assert(!G4 || (CH == 1 && G % 4 == 0), "gather4 path: 128-float slabs, whole quads per barrier group");
+                                                    float4* ring_all, uint64_t* bars_all) {
   constexpr int SLOT_V = CH * 32;                 // float4 per ring slot (one neighbour row of the slab)
   constexpr int SLOT_B = SLOT_V * 16;
   constexpr int D = BULK_RING / SLOT_B;           // ring depth in neighbour rows
@@ -629,17 +617,6 @@ __device__ __forceinline__ void spmm_chunk_cta_bulk(const SpmmParams& p, const i
       if ((jg & 31) == 0) { const int e = e_lo + jg + lane; cI = e < e_hi ? __ldg(p.col + e) : 0; }
       const int cnt = min(G, n - jg);
       const int u = lane - (jg & 31);
-      if (G4) {
-        // quads of 4 consecutive edges: the lane holding the first column index collects the other three (a ragged last
-        // quad repeats its first row; the surplus rows are never consumed)
-        const int c1 = __shfl_down_sync(FULL_MASK, cI, 1), c2 = __shfl_down_sync(FULL_MASK, cI, 2),
-                  c3 = __shfl_down_sync(FULL_MASK, cI, 3);
-        if (lane == 0) mbar_expect_tx(bars + b, (uint32_t)(((cnt + 3) >> 2) * 4 * SLOT_B));
-        if (u >= 0 && u < cnt && (u & 3) == 0)
-          tma_gather4(ring + (slot0 + u) * SLOT_V, tm, slab_voff * 4, cI, u + 1 < cnt ? c1 : cI, u + 2 < cnt ? c2 : cI,
-                      u + 3 < cnt ? c3 : cI, bars + b);
-        return;
-      }
       if (lane == 0) mbar_expect_tx(bars + b, (uint32_t)(cnt * SLOT_B));
       if (u >= 0 && u < cnt) {
         const float4* src = Xv + (size_t)cI * ldxv;
@@ -717,19 +694,6 @@ __device__ __forceinline__ void spmm_chunk_cta_bulk(const SpmmParams& p, const i
 }
 
 constexpr int BULK_SMEM = SPMM_WARPS * BULK_RING + SPMM_WARPS * BULK_MAX_GROUPS * 8;
-
-// gather4 variant: same kernel body, neighbour rows fetched four per TMA instruction through a tensor map of X
-template <int G, bool HAS_VAL, bool STATS>
-__global__ void __launch_bounds__(SPMM_THREADS, 3) spmm_rows_gather4_kernel(const __grid_constant__ CUtensorMap tm, const SpmmParams p) {
-  __shared__ float s_mem[2 * SPMM_MAX_SLAB_FLOATS];
-  extern __shared__ __align__(128) unsigned char s_dyn[];
-  const int per_slab = p.main_grid + p.n_seg;
-  const int slab = (int)blockIdx.x / per_slab;
-  const int b = (int)blockIdx.x - slab * per_slab;
-  if (b < p.n_seg) spmm_hub_seg_cta<float4, 1, HAS_VAL>(p, b, s_mem, slab, slab + 1);
-  else spmm_chunk_cta_bulk<1, G, HAS_VAL, STATS, true>(p, b - p.n_seg, slab, s_mem, reinterpret_cast<float4*>(s_dyn),
-                                                       reinterpret_cast<uint64_t*>(s_dyn + SPMM_WARPS * BULK_RING), &tm);
-}
 
 template <int CH, int G, bool HAS_VAL, bool STATS>
 __global__ void __launch_bounds__(SPMM_THREADS, 3) spmm_rows_bulk_kernel(const SpmmParams p) {
@@ -965,50 +929,6 @@ static int launch_spmm_bulk(const SpmmParams& p, cudaStream_t st, bool two_ctas)
   return B200GNN_OK;
 }
 
-// X [n_src, K] fp32 (row pitch ldx floats) as a 2-D tensor with {128 floats, 1 row} boxes: the gather4 source
-static bool make_gather_map(CUtensorMap* m, const float* X, int64_t n_src, int64_t K, int64_t ldx) {
-  tc::EncodeTiledFn fn = tc::encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)n_src};
-  cuuint64_t strides[1] = {(cuuint64_t)ldx * 4};
-  cuuint32_t box[2] = {128, 1};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(X), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <int G>
-static int launch_spmm_gather4(const SpmmParams& p, int64_t n_src, cudaStream_t st) {
-  CUtensorMap tm;
-  if (!make_gather_map(&tm, p.X, n_src, p.K, p.ldx)) return B200GNN_ERR_UNSUPPORTED;
-  int rc;
-  const bool stats = p.stat_partial != nullptr;
-  const int grid = (p.main_grid + p.n_seg) * p.n_slabs;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  static bool attr_done[64] = {};
-  if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(spmm_rows_gather4_kernel<G, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BULK_SMEM);
-    cudaFuncSetAttribute(spmm_rows_gather4_kernel<G, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BULK_SMEM);
-    cudaFuncSetAttribute(spmm_rows_gather4_kernel<G, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BULK_SMEM);
-    cudaFuncSetAttribute(spmm_rows_gather4_kernel<G, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BULK_SMEM);
-    attr_done[dev] = true;
-  }
-  if (p.val) {
-    if (stats) spmm_rows_gather4_kernel<G, true, true><<<grid, SPMM_THREADS, BULK_SMEM, st>>>(tm, p);
-    else spmm_rows_gather4_kernel<G, true, false><<<grid, SPMM_THREADS, BULK_SMEM, st>>>(tm, p);
-  } else {
-    if (stats) spmm_rows_gather4_kernel<G, false, true><<<grid, SPMM_THREADS, BULK_SMEM, st>>>(tm, p);
-    else spmm_rows_gather4_kernel<G, false, false><<<grid, SPMM_THREADS, BULK_SMEM, st>>>(tm, p);
-  }
-  if ((rc = check_launch())) return rc;
-  if (p.n_hub > 0) {
-    spmm_hub_finalize_kernel<<<p.n_hub, 256, 0, st>>>(p);
-    if ((rc = check_launch())) return rc;
-  }
-  return B200GNN_OK;
-}
-
 template <typename V>
 static int dispatch_ch(const SpmmParams& p, cudaStream_t st) {
   if (p.nvec <= 32) return launch_spmm<V, 1>(p, st);
@@ -1108,10 +1028,9 @@ static int g_spmm_variant = 0;
 struct ScatterArgs { int n; float* ptr[16]; int32_t off[17]; int64_t ld, col; };
 static thread_local ScatterArgs g_scatter = {0, {}, {}, 0, 0};
 
-// Slab width (floats) the bulk kernel uses when left to choose.  Measured on B200 (ARXIV-shape, profiles/r2_spmm_sweep):
-// the copy engine retires ~20 G row copies/s chip-wide whatever their size (tools/bulk_probe.cu), so narrower slabs
-// lose more to the per-copy cost than their L2 residency wins back (K=256: one 1 KB copy per neighbour 0.263 ms,
-// two 512 B slabs 0.37 ms): take the widest slab the ring supports.
+// Slab width (floats) the bulk kernel uses when left to choose: the widest slab the ring supports.  The copy engine
+// retires a roughly fixed number of row copies per second whatever their size (tools/bulk_probe.cu), so narrower slabs
+// pay more in per-copy cost than their L2 residency wins back.
 static int bulk_auto_slab(int64_t K, int64_t n_src) {
   (void)n_src;
   return (K % 256 == 0) ? 256 : 128;
@@ -1200,8 +1119,8 @@ extern "C" int b200gnn_spmm_csr_f32(const int32_t* rowptr, const int32_t* col, c
 
   // Variant word (b200gnn_spmm_set_variant; tuning and A/B tests): low nibble = kernel family
   //   0 automatic, 1 register-staged, 2 cp.async ring (round-1 kernel), 3 bulk-copy ring, one slab of min(K,256) floats
-  //   per pass, 4 bulk-copy ring with 128-float slabs, 5 bulk-copy ring with 256-float slabs, 6 / 7 TMA gather4 quads over
-  //   128-float slabs (8 / 4 edges per barrier group);
+  //   per pass, 4 bulk-copy ring with 128-float slabs, 5 bulk-copy ring with 256-float slabs, 6 / 7 bulk-copy ring
+  //   with 128-float slabs and 8 / 4 edges per barrier group;
   //   +16 = evict_last L2 policy on the gathers, +32 = the other barrier-group size, +64 = 2 CTAs per SM.
   const int fam = g_spmm_variant & 15;
   const bool alt_g = (g_spmm_variant & 32) != 0;
@@ -1210,7 +1129,7 @@ extern "C" int b200gnn_spmm_csr_f32(const int32_t* rowptr, const int32_t* col, c
     if (fam == 3) bulk_sw = (K % 256 == 0) ? 256 : 128;
     else if (fam == 4) bulk_sw = 128;
     else if (fam == 5) bulk_sw = (K % 256 == 0) ? 256 : 128;
-    else if (fam == 6 || fam == 7) bulk_sw = 128;        // gather4 quads of 128-float slab rows (6: 8 edges per barrier, 7: 4)
+    else if (fam == 6 || fam == 7) bulk_sw = 128;
     else if (fam == 0) bulk_sw = bulk_auto_slab(K, n_src);
   }
   int rc;
@@ -1219,11 +1138,8 @@ extern "C" int b200gnn_spmm_csr_f32(const int32_t* rowptr, const int32_t* col, c
   if (bulk_sw) {
     p.n_slabs = (int32_t)(K / bulk_sw);
     p.l2_hint = (g_spmm_variant & 16) ? 1 : 0;
-    // automatic choice (measured, ARXIV-shape, profiles/r2_spmm_sweep.jsonl): one 128-float slab -> gather4 quads
-    // (K=128: 0.153 ms against 0.198 for single-row copies); wider rows -> one 1 KB copy per neighbour (K=256: 0.263 ms;
-    // two gather4 slab passes cost 0.28: the pass count outweighs the L2 residency)
-    if (fam == 6 || (fam == 0 && K == 128)) return launch_spmm_gather4<8>(p, n_src, st);
-    if (fam == 7) return launch_spmm_gather4<4>(p, n_src, st);
+    if (fam == 6) return launch_spmm_bulk<1, 8>(p, st, false);
+    if (fam == 7) return launch_spmm_bulk<1, 4>(p, st, false);
     const bool two = (g_spmm_variant & 64) != 0;    // +64: two CTAs per SM instead of three
     if (bulk_sw == 128) rc = alt_g ? launch_spmm_bulk<1, 2>(p, st, two) : launch_spmm_bulk<1, 4>(p, st, two);
     else rc = alt_g ? launch_spmm_bulk<2, 2>(p, st, two) : launch_spmm_bulk<2, 4>(p, st, two);

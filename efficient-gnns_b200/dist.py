@@ -1,7 +1,7 @@
 """Node-parallel full-batch training across P GPUs (SURVEY.md §8e; BASELINE.json north_star).
 
 The reference is single-GPU (one process per `--device`, arxiv_pyg/scripts/run_gcn.sh:24-28); this is the
-B200-native extension the north star asks for, and its correctness target is equality with the 1-GPU step.
+native multi-GPU extension the north star asks for, and its correctness target is equality with the 1-GPU step.
 
 Partition
     Nodes are relabelled by a degree-balancing permutation (sort by degree, deal out in snake order) so that P

@@ -10,6 +10,8 @@ import os
 import torch
 import torch.distributed as dist
 
+NVLINK_GBS = 450.0      # H100 SXM data sheet: NVLink 4, GB/s per direction per GPU
+
 
 def run(args):
     import bench as B
@@ -152,18 +154,18 @@ def run(args):
                     else f"node-parallel x{world}: degree-balanced row blocks, one NCCL all-gather per aggregation",
                     "dist_mode": mode,
                     "cuda_graph": bool(graph), "exchange_bytes_received_per_rank_per_step": ex,
-                    "nvlink_floor_ms": ex / 770e9 * 1e3,
+                    "nvlink_floor_ms": ex / NVLINK_GBS / 1e6,
                     "aggregations_executed": tr.aggregations_per_step()},
                 "roofline": {"bound": "nvlink+hbm",
                              "note": ("multi-GPU point. achieved = bytes each rank RECEIVES over NVLink per step / step time against the "
-                                      "measured 770 GB/s peer bandwidth (nvlink_floor_ms = the same bytes at that rate). For the hybrid "
+                                      "H100 SXM data sheet's 450 GB/s per direction of NVLink 4 (nvlink_floor_ms = the same bytes at that rate). For the hybrid "
                                       "layout the exchanges are stores issued by the producing kernels' epilogues and the floor is far "
                                       "below the step: the limiter is the per-rank compute that does not shrink with N (every rank "
-                                      "walks all edges at width K/N; profiles/r2_hybrid_rank_w*_summary.txt), not the links")
+                                      "walks all edges at width K/N; tools/profile_hybrid_rank.py measures it), not the links")
                              if mode.startswith("hybrid") else
                              "multi-GPU point: the all-gathers bound the step; see nvlink_floor_ms",
-                             "achieved": ex / (ms_step * 1e-3) / 1e9, "peak": 770.0, "unit": "GB/s",
-                             "frac": ex / (ms_step * 1e-3) / 1e9 / 770.0, "traffic": None},
+                             "achieved": ex / (ms_step * 1e-3) / 1e9, "peak": NVLINK_GBS, "unit": "GB/s",
+                             "frac": ex / (ms_step * 1e-3) / 1e9 / NVLINK_GBS},
                 "cpu_baseline": None,
                 "e2e": {"value": 6 * nnz / (ms_e2e * 1e-3), "unit": B.UNIT, "ms_per_step": ms_e2e,
                         "h2d_bytes_per_step": h2d * world, "d2h_bytes_per_step": 12 * world},

@@ -11,7 +11,7 @@ Mirrors what one call of the reference's ``train()`` does for ``--gnn gcn --trai
     Adam over one flat parameter buffer.
 
 No autograd tape: activations live in preallocated buffers and the whole step (≈40 launches) is captured
-into one CUDA graph.  Everything except the three GEMM shapes is hand-written sm_100a code behind the C ABI.
+into one CUDA graph.  Everything except the three GEMM shapes is hand-written sm_90a code behind the C ABI.
 """
 from __future__ import annotations
 
@@ -115,14 +115,14 @@ class GCNStudentTrainer:
                 g, gg = take(dims[l + 1], (dims[l + 1],))
                 be, gbe = take(dims[l + 1], (dims[l + 1],))
                 self.gamma.append(g); self.ggamma.append(gg); self.beta.append(be); self.gbeta.append(gbe)
-        # tf32 hi/lo splits of the weights for the tcgen05 GEMM: W^T [out,in] feeds the forward (C = X W),
+        # tf32 hi/lo splits of the weights for the wgmma GEMM: W^T [out,in] feeds the forward (C = X W),
         # W [in,out] feeds the input gradient (dX = dH W^T); refreshed every step (a few KB).
         self.Wt_split = [(torch.empty(dims[l + 1], dims[l], device=dev), torch.empty(dims[l + 1], dims[l], device=dev))
                          for l in range(self.L)]
         self.W_split = [(torch.empty(dims[l], dims[l + 1], device=dev), torch.empty(dims[l], dims[l + 1], device=dev))
                         for l in range(self.L)]
         wg = [ops.wgrad_supported(dims[l], dims[l + 1]) for l in range(self.L)]
-        self.wgrad_ws = (torch.empty(148 * max(dims[l] * ((dims[l + 1] + 31) // 32 * 32) for l in range(self.L) if wg[l]), device=dev)
+        self.wgrad_ws = (torch.empty(max(ops.wgrad_workspace_floats(dims[l], dims[l + 1]) for l in range(self.L) if wg[l]), device=dev)
                          if self.tc_gemm and any(wg) else None)
         self.running_mean = [torch.zeros(d, device=dev) for d in dims[1:-1]]
         self.running_var = [torch.ones(d, device=dev) for d in dims[1:-1]]
@@ -312,7 +312,7 @@ class GCNStudentTrainer:
             torch.cuda.current_stream().wait_event(self._ev_join)
 
     def _linear(self, l: int, inp: torch.Tensor, out: torch.Tensor, bias: Optional[torch.Tensor] = None):
-        """out = inp @ W_l (+bias): tcgen05 3xTF32 kernel, or cuBLAS fp32 when disabled."""
+        """out = inp @ W_l (+bias): wgmma 3xTF32 kernel, or cuBLAS fp32 when disabled."""
         if self.tc_gemm:
             hi, lo = ops.split_tf32(self.W[l], transpose=True, hi=self.Wt_split[l][0], lo=self.Wt_split[l][1])
             ops.gemm_tf32x3(inp, hi, lo, bias=bias, out=out)
@@ -332,7 +332,7 @@ class GCNStudentTrainer:
             torch.mm(d_out, self.W[l].t(), out=d_inp)
 
     def _linear_wgrad(self, l: int, inp: torch.Tensor, d_out: torch.Tensor):
-        """grad W_l = inp^T @ d_out: split-K tcgen05 kernel where the tiling allows, cuBLAS fp32 otherwise."""
+        """grad W_l = inp^T @ d_out: split-K wgmma kernel where the tiling allows, cuBLAS fp32 otherwise."""
         if self.tc_gemm and ops.wgrad_supported(self.dims[l], self.dims[l + 1]):
             ops.gemm_wgrad_tf32x3(inp, d_out, out=self.gW[l], workspace=self.wgrad_ws)
         else:

@@ -4,11 +4,11 @@
 Per layer (PyG SAGEConv: aggregate first, no self loops, unweighted mean):
 
     M  = mean_{j in N(i)} X_j                       b200gnn SpMM (mean), TMA kernels at these widths
-    Y  = M W_l^T + b_l + X W_r^T                    two tcgen05 GEMMs, the second through the ACCUMULATING epilogue
+    Y  = M W_l^T + b_l + X W_r^T                    two wgmma GEMMs, the second through the ACCUMULATING epilogue
     X' = dropout(relu(BN(Y)))                       hidden layers; column statistics + the fused pass of dense_rows.cu
 backward:
     dM = dY W_l ;  dX = dY W_r + A_mean^T dM        (SpMM on the cached 1/deg-weighted CSC view, GEMM accumulating on top)
-    dW_l = dY^T M, dW_r = dY^T X, db_l = colsum dY  split-K tcgen05 weight-gradient GEMMs where the tiling allows
+    dW_l = dY^T M, dW_r = dY^T X, db_l = colsum dY  split-K wgmma weight-gradient GEMMs where the tiling allows
     Adam over one flat parameter buffer.
 
 No autograd tape, no torch BatchNorm / Adam, no cuBLAS on the step where the tensor-core tilings apply (round 1 ran SAGE
@@ -91,7 +91,7 @@ class SAGEStudentTrainer:
         self.kd_part = torch.empty(2 * int(lib.load().b200gnn_kd_partials(N)), device=dev)
         self.split = {}
         wg = [(dims[l], dims[l + 1]) for l in range(self.L) if ops.wgrad_supported(dims[l], dims[l + 1])]
-        self.wgrad_ws = torch.empty(148 * max(a * ((b + 31) // 32 * 32) for a, b in wg), device=dev) if wg else None
+        self.wgrad_ws = torch.empty(max(ops.wgrad_workspace_floats(a, b) for a, b in wg), device=dev) if wg else None
         self.loss_aux = None
         self._graph = None
         self.reset_parameters(seed)

@@ -1,4 +1,4 @@
-"""Hybrid-layout multi-GPU training step (SURVEY.md §8e; BASELINE.json north_star "up to 8 B200s").
+"""Hybrid-layout multi-GPU training step (SURVEY.md §8e; BASELINE.json north_star "up to 8 H100s").
 
 Why not plain node parallelism.  Row-sharding Â makes every aggregation all-gather its whole [N, K] operand: on a graph
 without locality each rank references ~all rows, so at P = 8 every rank RECEIVES 7/8 of two [N,256] tensors per step

@@ -1,4 +1,4 @@
-"""GAT teacher layer across P GPUs (BASELINE.json configs[3] "GAT teacher 8-head edge-softmax ... 1→8×B200"; SURVEY.md §8e).
+"""GAT teacher layer across P GPUs (BASELINE.json configs[3] "GAT teacher 8-head edge-softmax ... 1→8×H100"; SURVEY.md §8e).
 
 SURVEY §8e sketched a node-parallel scheme with a source-side halo of ``ft`` and ``el`` and a non-symmetric backward.  The
 hybrid layout of hybrid.py makes all of that unnecessary: attention is computed PER HEAD, so with the columns of the projected
@@ -8,7 +8,7 @@ the symmetric degree scaling, and their hand-written backward (csrc/gat.cu) — 
 whole (replicated, 30 MB) graph with NO halo and no cross-rank reduction.  Only the dense projections stay node-parallel
 ("R layout"), and the two layouts are connected by the same R<->C exchanges as the GCN engine:
 
-    feat_R ──fc (tcgen05)──▶ ft_R [n_p, H·D] ──R→C──▶ ft_C [N, (H/P)·D] ──attention + aggregation on own heads──▶ rst_C ──C→R──▶ rst_R
+    feat_R ──fc (wgmma)──▶ ft_R [n_p, H·D] ──R→C──▶ ft_C [N, (H/P)·D] ──attention + aggregation on own heads──▶ rst_C ──C→R──▶ rst_R
     rst_R += res_fc(feat_R)                                                                       (models.py:228-230)
 
 Exchanged per layer and direction: N·H·D·4·(P−1)/P² bytes per rank (8× less than gathering ``ft`` at P = 8).  Autograd:

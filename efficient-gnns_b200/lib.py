@@ -81,7 +81,6 @@ SIGNATURES = {
     "b200gnn_gemm_tf32x3_scatter_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gemm_tf32x3_bcast_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_wgrad_workspace_floats": (_i64, [_i64, _i64]),
-    "b200gnn_wgrad_set_mode": (None, [_int]),
     "b200gnn_gemm_wgrad_tf32x3_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_row_normalize_fwd_f32": (_int, [_f32p, _i64, _i64, _f32, _f32, _f32p, _f32p, _ptr]),
     "b200gnn_row_normalize_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _f32, _f32p, _int, _ptr]),
@@ -143,13 +142,13 @@ def load() -> C.CDLL:
     if not LIB_PATH.exists():
         raise B200GnnError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU or PyTorch fallback for the b200gnn operators.")
+            "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the b200gnn operators.")
     lib = C.CDLL(str(LIB_PATH))
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError => ABI mismatch, fail loudly
         fn.restype = res
         fn.argtypes = args
-    if lib.b200gnn_abi_version() != 1:
+    if lib.b200gnn_abi_version() != 2:
         raise B200GnnError("libb200gnn.so ABI version mismatch; rebuild")
     _lib = lib
     report = os.environ.get("B200GNN_LAUNCH_REPORT")

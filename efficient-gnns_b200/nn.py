@@ -7,7 +7,7 @@
 
 Parameter names and shapes follow PyG 1.6/1.7 (``GCNConv.weight`` is [in, out], ``SAGEConv.lin_l/lin_r`` are
 ``nn.Linear``), so ``state_dict``s are interchangeable with the reference's checkpoints.
-Dense contractions run on the tcgen05 3xTF32 GEMMs, aggregations on the CSR SpMM; both are differentiable.
+Dense contractions run on the wgmma 3xTF32 GEMMs, aggregations on the CSR SpMM; both are differentiable.
 """
 from __future__ import annotations
 
@@ -181,7 +181,7 @@ class DGLGraphConv(torch.nn.Module):
     ``out = D_in^-1/2 A D_out^-1/2 x W + b`` with degrees clamped to >= 1 and no self-loops added (the script adds them to the
     graph).  Called as ``conv(adj_t, feat)`` with a SparseTensor (row = destination, col = source) in place of the DGL graph.
     The two degree scalings are folded into the edge values once per adjacency, so the layer is one weighted SpMM and one
-    tcgen05 GEMM; like DGL the narrower side is aggregated (W first iff in > out)."""
+    wgmma GEMM; like DGL the narrower side is aggregated (W first iff in > out)."""
 
     def __init__(self, in_feats, out_feats, norm="both", weight=True, bias=True, activation=None):
         super().__init__()

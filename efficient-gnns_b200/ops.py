@@ -257,7 +257,7 @@ def kd_loss_fwd_bwd(logits, labels, train_idx, teacher_logits=None, alpha: float
     return loss_out, d_logits
 
 
-# ----------------------------------------------------------------------------- tcgen05 3xTF32 GEMM
+# ----------------------------------------------------------------------------- wgmma 3xTF32 GEMM
 def split_tf32(w: torch.Tensor, transpose: bool = False, hi: Optional[torch.Tensor] = None,
                lo: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """(hi, lo) tf32 split of a small [rows, cols] matrix; transposed ([cols, rows]) output if requested."""
@@ -358,6 +358,11 @@ def gemm_tf32x3_bcast(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, d
 
 def wgrad_supported(k_in: int, n_out: int) -> bool:
     return k_in in (128, 256) and n_out % 4 == 0 and 0 < n_out <= 256
+
+
+def wgrad_workspace_floats(k_in: int, n_out: int) -> int:
+    """Size of the workspace gemm_wgrad_tf32x3 fills (fp32 elements)."""
+    return int(lib.load().b200gnn_wgrad_workspace_floats(k_in, n_out))
 
 
 def gemm_wgrad_tf32x3(x: torch.Tensor, g: torch.Tensor, out: Optional[torch.Tensor] = None,

@@ -1,5 +1,5 @@
 """Full-batch R-GCN engine — ``RGCN.inference`` of the reference (mag_pyg/gnn.py:140-171), BASELINE.json configs[4]
-("R-GCN teacher ... MAG-shape heterogeneous ... node-parallel 2/4/8×B200").
+("R-GCN teacher ... MAG-shape heterogeneous ... node-parallel 2/4/8×H100").
 
 Per layer and node type t (the reference's loop, :153-169):
 
@@ -10,7 +10,7 @@ Per layer and node type t (the reference's loop, :153-169):
 
 What differs from the reference's execution (not from its arithmetic): the per-relation CSR is built ONCE by the device
 ingestion kernels (the reference re-sorts every relation on every call, :149-151); the relation GEMMs add into ``out[t]``
-through the accumulating tcgen05 epilogue (``b200gnn_gemm_tf32x3_acc_f32``) instead of materialising ``rel_lins(tmp)`` and
+through the accumulating wgmma epilogue (``b200gnn_gemm_tf32x3_acc_f32``) instead of materialising ``rel_lins(tmp)`` and
 an ``add_``; aggregation runs before the transform, as in the reference's inference (its training path transforms per EDGE).
 
 Multi-GPU (``exchange`` given): same hybrid layout as hybrid.py, per node type — activations live node-parallel ("R": rank p
@@ -77,7 +77,7 @@ class RGCNInference:
 
     # ------------------------------------------------------------------ helpers
     def _gemm(self, x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, bias=None, accumulate=False):
-        """out (+)= x @ w^T (+bias) on the tcgen05 GEMM; K not a multiple of 4 is zero-padded (exact)."""
+        """out (+)= x @ w^T (+bias) on the wgmma GEMM; K not a multiple of 4 is zero-padded (exact)."""
         k = x.shape[1]
         if k % 4:
             pad = 4 - k % 4

@@ -3,7 +3,7 @@
 There is no network for ogbn-arxiv / ogbn-mag, so the benchmark and the tests use
 graphs with the same node/edge counts, feature widths and a citation-like heavy
 in-degree tail.  Everything is generated on the CPU with an explicit
-``torch.Generator`` so the GPU box and this container produce identical inputs.
+``torch.Generator`` so every machine produces identical inputs.
 """
 from __future__ import annotations
 

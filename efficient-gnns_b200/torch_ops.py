@@ -9,7 +9,7 @@ This module registers the same stateless forms under the `b200gnn` namespace wit
     torch.ops.b200gnn.spmm_mean(rowptr, col, value?, mat) -> Tensor      row-mean (A.4: divide by the row's entry count)
     torch.ops.b200gnn.ind2ptr  (ind, M) -> Tensor / ptr2ind(ptr, E) -> Tensor
     torch.ops.b200gnn.split_tf32(w, transpose) -> (hi, lo)
-    torch.ops.b200gnn.gemm_tf32x3(a, b_hi, b_lo, bias?) -> Tensor        fp32-faithful tcgen05 GEMM  a · bᵀ (+bias)
+    torch.ops.b200gnn.gemm_tf32x3(a, b_hi, b_lo, bias?) -> Tensor        fp32-faithful wgmma GEMM  a · bᵀ (+bias)
 
 Each has a fake (meta) implementation, so the ops trace under `torch.compile` / FakeTensorMode, and the two SpMMs carry
 autograd (gradient w.r.t. `mat`: the same kernel on the transposed matrix, upstream's spmm backward).  int64 indices at the

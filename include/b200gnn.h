@@ -1,11 +1,11 @@
 /*
- * b200gnn.h — C ABI of the B200-native sparse message-passing engine.
+ * b200gnn.h — C ABI of the H100-native (sm_90a) sparse message-passing engine.
  *
  * This is the drop-in boundary for the hot path of chaitjo/efficient-gnns
  * (SURVEY.md §8b).  The reference reaches its sparse arithmetic through
  * un-vendored Python/C++ dependencies (torch_sparse / torch_scatter / PyG);
  * each entry point below names the reference call site (file:line, relative
- * to /root/reference) whose arithmetic it replaces.
+ * to the reference repository's root) whose arithmetic it replaces.
  *
  * Conventions
  *   - All pointers are DEVICE pointers unless the name ends in `_host`.
@@ -38,7 +38,7 @@ extern "C" {
 #define B200GNN_REDUCE_SUM 0
 #define B200GNN_REDUCE_MEAN 1
 
-#define B200GNN_ABI_VERSION 1
+#define B200GNN_ABI_VERSION 2
 
 int b200gnn_abi_version(void);
 const char* b200gnn_error_string(int code);
@@ -250,8 +250,8 @@ int b200gnn_kd_loss_fwd_bwd_f32(const float* logits, int64_t ld,
                                 float* loss_out, float* partial, void* stream);
 
 /* ------------------------------------------------------------------ *
- * fp32-faithful dense GEMM on tcgen05 tensor cores (3xTF32 split, fp32
- * accumulation in TMEM):   C[M,N] = A[M,K] * B[N,K]^T (+ bias[N])
+ * fp32-faithful dense GEMM on the Hopper tensor cores (wgmma, 3xTF32 split,
+ * fp32 accumulation in registers):   C[M,N] = A[M,K] * B[N,K]^T (+ bias[N])
  * Replaces the fp32 cuBLAS contractions behind GCNConv's `x @ weight`,
  * nn.Linear and their input gradients (arxiv_pyg/gnn.py:47,52,79,84 via PyG).
  *   A    : fp32, row-major, split into tf32 hi/lo on the fly inside the kernel.
@@ -271,7 +271,7 @@ int b200gnn_gemm_tf32x3_acc_f32(const float* A, int64_t lda, const float* B_hi, 
                                 int64_t ldb, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
                                 void* stream);
 /* Row passes fused into the GEMM epilogue (SURVEY §8 f1; the reference runs conv -> BatchNorm1d -> ReLU -> dropout as
- * separate full-matrix ops, arxiv_pyg/gnn.py:47-50, and autograd walks them again backwards).  Each epilogue warp keeps
+ * separate full-matrix ops, arxiv_pyg/gnn.py:47-50, and autograd walks them again backwards).  Each consumer warp keeps
  * running column sums over the tiles of its CTA and stores them once: partial[slots][2][N], slots >=
  * b200gnn_gemm_stat_slots(M, N), fixed summation order (deterministic).  N a multiple of 32, 48 < N <= 256, ldc % 4 == 0.
  *   _stats_f32 : C = A·B^T + bias (accumulate: C += A·B^T, no bias — SAGEConv's lin_l(mean) + lin_r(x)) and partial = per-slot (sum C, sum C^2) over rows — the BatchNorm batch statistics of C,
@@ -282,8 +282,8 @@ int b200gnn_gemm_tf32x3_acc_f32(const float* A, int64_t lda, const float* B_hi, 
  *                b200gnn_bn_act_bwd_reduce_f32; follow with b200gnn_bn_act_bwd_apply_f32(dOut = C, Xout = NULL, sums =
  *                partial)).  Xout, Y: [M, ldc] like C. */
 int64_t b200gnn_gemm_stat_slots(int64_t M, int64_t N);
-/* A/B knob for measurements: 0 automatic (Xout / Y of _bnbwd_f32 staged through TMA when N % 128 == 0), 2 = always the
- * register path. */
+/* A/B knob for measurements: 0 automatic (Xout / Y of _bnbwd_f32 staged through TMA when N % 128 == 0 and K < 128),
+ * 1 = the TMA path whenever N % 128 == 0, 2 = always the register path. */
 void b200gnn_gemm_set_bnbwd_variant(int v);
 int b200gnn_gemm_tf32x3_stats_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
                                   float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
@@ -306,7 +306,7 @@ int b200gnn_gemm_tf32x3_bcast_f32(const float* A, int64_t lda, const float* B_hi
                                   int64_t M, int64_t N, int64_t K, const float* bias, void* stream);
 
 /* Weight gradient  dW[Kin,Nout] = X[Nn,Kin]^T * G[Nn,Nout]  (GCNConv weight.grad / nn.Linear weight.grad^T),
- * split-K over the node index on tcgen05 (3xTF32), partials reduced in fixed order.
+ * split-K over the node index on the Hopper tensor cores (wgmma, 3xTF32), partials reduced in fixed order.
  * Kin in {128,256}, Nout a multiple of 4 up to 256 (else B200GNN_ERR_UNSUPPORTED: caller keeps the library GEMM).
  * workspace: float[b200gnn_wgrad_workspace_floats(Kin,Nout)]. */
 int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout);
@@ -314,9 +314,6 @@ int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G,
                                   int64_t ldg, float* dW, int64_t Nn,
                                   int64_t Kin, int64_t Nout, float* workspace,
                                   void* stream);
-/* A/B knob for measurements: 0 automatic (separate correction accumulators / drains against the accumulator's
- * round-towards-zero), 1 drains only, 2 one accumulation chain per CTA (round-1 behaviour, 1e-5-level gradient error). */
-void b200gnn_wgrad_set_mode(int mode);
 
 /* ------------------------------------------------------------------ *
  * Feature-distillation criteria (arxiv_pyg/criterion.py): row / pair passes.

@@ -3,7 +3,7 @@
 A plain numpy / PyTorch-CPU restatement of the algorithms on the hot path of
 chaitjo/efficient-gnns (SURVEY.md §8a, Appendix A).  The arithmetic of that path
 lives in third-party, un-vendored dependencies that are absent from
-/root/reference and not installable here (no network):
+the reference repository and not installed here:
     torch-geometric 1.6.x-1.7.x, torch-sparse 0.6.8-0.6.10, torch-scatter 2.0.5-2.0.7,
     dgl 0.5-0.6, torch 1.7.1                                   (README.md:37-66)
 so their published semantics are restated here, each function citing the

@@ -2,7 +2,7 @@
 
 The reference drives `torch_geometric.data.GraphSAINTRandomWalkSampler(homo_data, batch_size, walk_length=num_layers,
 num_steps, sample_coverage=0)` at mag_pyg/gnn.py:361-366 and consumes its batches at :187-190.  The algorithm itself lives in
-third-party packages that are NOT vendored under /root/reference (torch_geometric 1.x `GraphSAINTSampler.__getitem__ /
+third-party packages that are NOT vendored in the reference repository (torch_geometric 1.x `GraphSAINTSampler.__getitem__ /
 __collate__`, torch_sparse `random_walk` and `SparseTensor.saint_subgraph`; versions per the reference README: PyG 1.6.x,
 torch_sparse 0.6.x), so it is restated here from their published behaviour:
 

@@ -1,8 +1,8 @@
 """Generate golden fixtures by running the REFERENCE's own Python files, unmodified, in the build container.
 
-    python tests/golden/make_golden.py        (needs /root/reference; not run on the GPU box)
+    python tests/golden/make_golden.py        REFERENCE=<checkout of the reference repository>   (not run by the test suite)
 
-/root/reference's hot-path arithmetic lives in torch_geometric / torch_sparse, which are not installed,
+The reference's hot-path arithmetic lives in torch_geometric / torch_sparse, which are not installed,
 so `arxiv_pyg/criterion.py` and `arxiv_pyg/gnn.py` are imported on top of minimal stand-in modules whose
 operators come from oracle/ (the CPU restatement).  What the fixtures therefore pin:
   * criterion_*.pt  — outputs/gradients of the reference's six criteria (kd, fitnet, at, gpw, lpw, nce)
@@ -26,6 +26,7 @@ from __future__ import annotations
 
 import importlib
 import importlib.util
+import os
 import sys
 import types
 from pathlib import Path
@@ -35,7 +36,7 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[2]
 sys.path.insert(0, str(ROOT))
-REF = Path("/root/reference")
+REF = Path(os.environ.get("REFERENCE", "reference"))
 OUT = Path(__file__).resolve().parent
 
 from oracle import graph as og, ops as oo  # noqa: E402
@@ -227,7 +228,7 @@ def small_graph(n=240, e=1400, seed=3):
 
 
 def main():
-    assert REF.exists(), "/root/reference is needed to regenerate the fixtures"
+    assert REF.exists(), "set REFERENCE to a checkout of the reference repository to regenerate the fixtures"
     install_stubs()
     sys.path.insert(0, str(REF / "arxiv_pyg"))
     crit = importlib.import_module("criterion")

@@ -1,7 +1,7 @@
 """Round-2 golden fixtures: the reference's OWN files at sizes that cross the engine's special paths (hub rows split
 across CTAs, the pipelined K=256 kernel, the 750-wide teacher features) and the PPI criterion file.
 
-    python tests/golden/make_golden_r2.py        (needs /root/reference; not run on the GPU box)
+    python tests/golden/make_golden_r2.py        REFERENCE=<checkout of the reference repository>   (not run by the test suite)
 
 Same method as make_golden.py (whose stand-in modules are reused): the reference file computes, the third-party
 primitives underneath come from oracle/.  Large outputs are stored for a fixed subset of rows (`rows`) plus their full

@@ -28,7 +28,7 @@ def test_python_signature_table_matches_header():
 
 def test_abi_version_and_error_strings():
     L = lib.load()
-    assert L.b200gnn_abi_version() == 1
+    assert L.b200gnn_abi_version() == 2
     assert L.b200gnn_error_string(0) == b"ok"
     assert b"argument" in L.b200gnn_error_string(-1)
     assert L.b200gnn_spmm_stat_slots(17, 3) == 3 + 3

@@ -1,5 +1,5 @@
 """bench.py's output contract, checked on the CPU-only arm (`--impl reference`): exactly one line on stdout, valid JSON,
-the keys the driver reads.  (The GPU arm prints the same keys plus roofline / clocks; it is exercised on the GPU box.)"""
+the keys a consumer reads.  (The GPU arm prints the same keys plus roofline / clocks; it is exercised on the GPU.)"""
 import json
 import subprocess
 import sys
@@ -34,3 +34,10 @@ def test_reference_arm_is_silent_on_non_zero_ranks():
     p = subprocess.run([sys.executable, str(ROOT / "bench.py"), "--impl", "reference", "--gpus", "2", "--steps", "1"],
                        capture_output=True, text=True, timeout=120, cwd=str(ROOT), env=env)
     assert p.returncode == 0 and p.stdout.strip() == ""
+
+
+def test_dump_outputs_is_rejected_for_the_reference_arm(tmp_path):
+    p = subprocess.run([sys.executable, str(ROOT / "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "0",
+                        "--dump-outputs", str(tmp_path / "d")], capture_output=True, text=True, timeout=120, cwd=str(ROOT))
+    assert p.returncode == 2 and p.stdout.strip() == "", p.stderr[-2000:]
+    assert "--dump-outputs" in p.stderr and not (tmp_path / "d").exists()

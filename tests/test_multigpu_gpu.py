@@ -1,5 +1,5 @@
-"""Multi-rank equivalence inside the driver-run GPU suite: spawns torchrun on 2 (and 4) GPUs of the box when they are
-visible and skips otherwise (the single-GPU boxes of the regular run).  The scripts compare the P-GPU step with the
+"""Multi-rank equivalence inside the GPU suite: spawns torchrun on 2 (and 4) GPUs of the machine when they are
+visible and skips otherwise (single-GPU machines).  The scripts compare the P-GPU step with the
 1-GPU engine on the same inputs (tests/hybrid_equiv.py, tests/dist_equiv.py)."""
 import os
 import socket

@@ -1,5 +1,5 @@
 """R-GCN on the mirrored PyG surface (MessagePassing.propagate with mean aggregation, SparseTensor.matmul(reduce='mean'),
-tcgen05 Linear) against the fixture produced by the reference's own RGCN / RGCNConv classes (mag_pyg/gnn.py:26-171,
+wgmma Linear) against the fixture produced by the reference's own RGCN / RGCNConv classes (mag_pyg/gnn.py:26-171,
 tests/golden/make_golden.py).  The module tree below only re-creates the parameter layout the fixture's state_dict names."""
 import pytest
 import torch
@@ -120,7 +120,7 @@ def test_group_input_typed_gather_and_deterministic_scatter():
 
 def test_full_batch_rgcn_engine_matches_reference_inference_fixture(golden_rgcn):
     """efficient_gnns_b200.rgcn.RGCNInference (relation CSRs built once by the ingestion kernels, aggregate-then-transform with
-    the accumulating tcgen05 epilogue) vs the output of the reference's own RGCN.inference (mag_pyg/gnn.py:140-171)."""
+    the accumulating wgmma epilogue) vs the output of the reference's own RGCN.inference (mag_pyg/gnn.py:140-171)."""
     from efficient_gnns_b200.rgcn import RGCNInference
     G = golden_rgcn
     eng = RGCNInference(G["state"], G["num_nodes"], G["edge_index_dict"], G["key2int"])

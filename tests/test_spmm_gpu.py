@@ -171,7 +171,7 @@ def test_large_arxiv_shape_properties():
 
 # ---------------------------------------------------------------------------------------------- round 2: bulk-copy kernel
 # variant word: 2 = cp.async ring, 3 = bulk (slab min(K,256)), 4 = bulk 128-float slabs, 5 = bulk 256-float slabs,
-# 6 / 7 = TMA gather4 quads over 128-float slabs (8 / 4 edges per barrier), +16 evict_last gathers, +32 other barrier-group
+# 6 / 7 = bulk-copy ring over 128-float slabs with 8 / 4 edges per barrier, +16 evict_last gathers, +32 other barrier-group
 # size, +64 two CTAs per SM (efficient-gnns_b200/csrc/spmm.cu)
 BULK_VARIANTS = [0, 1, 2, 3, 4, 5, 6, 7, 3 + 16, 4 + 16, 3 + 32, 4 + 32, 5 + 16 + 32, 3 + 64]
 

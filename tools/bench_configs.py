@@ -188,7 +188,7 @@ def main():
         xp = torch.randn(synthetic.MAG_NODES[types[0]], 128, generator=g).to(dev)
         ms = med_time(lambda: eng({0: xp}), 5, 2)
         print(json.dumps(dict(config=5, what=f"MAG-shape full-batch R-GCN inference, 2 layers 128->{hidden}->349: 14 rectangular mean-SpMMs + "
-                                             "22 tcgen05 GEMMs (relation GEMMs accumulate in the epilogue), CSRs built once",
+                                             "22 wgmma GEMMs (relation GEMMs accumulate in the epilogue), CSRs built once",
                               relations=len(rels), nnz_total=eng.nnz, ms=ms, edges_per_s=2 * eng.nnz / ms * 1e3)), flush=True)
         del eng, state
         torch.cuda.empty_cache()

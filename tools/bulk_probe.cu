@@ -1,6 +1,6 @@
 // Micro-probe for the SpMM data path: random row gathers with cp.async.bulk (UBLKCP) into per-warp shared-memory rings,
 // completion on mbarriers, rows summed from shared memory (what the aggregation kernel does, without the CSR walk).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a tools/bulk_probe.cu -o /tmp/bulk_probe && /tmp/bulk_probe
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a tools/bulk_probe.cu -o /tmp/bulk_probe && /tmp/bulk_probe
 // Sweeps table size (L2-resident .. DRAM), row bytes (256 / 512 / 1024), ring bytes per warp and CTAs per SM.
 #include <cstdio>
 #include <cstdint>
@@ -90,9 +90,9 @@ static void run(const char* X, size_t tb, const int* d_idx, int n_idx, float4* s
   const int smem = 8 * RING + 8 * (RING / RB / G) * 8;
   cudaFuncSetAttribute(bulk_gather<RB, RING, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-  bulk_gather<RB, RING, G><<<148 * ctas_per_sm, 256, smem>>>(X, d_idx, n_idx, sink);
+  bulk_gather<RB, RING, G><<<132 * ctas_per_sm, 256, smem>>>(X, d_idx, n_idx, sink);
   cudaEventRecord(a);
-  for (int it = 0; it < 5; ++it) bulk_gather<RB, RING, G><<<148 * ctas_per_sm, 256, smem>>>(X, d_idx, n_idx, sink);
+  for (int it = 0; it < 5; ++it) bulk_gather<RB, RING, G><<<132 * ctas_per_sm, 256, smem>>>(X, d_idx, n_idx, sink);
   cudaEventRecord(b); cudaEventSynchronize(b);
   float ms; cudaEventElapsedTime(&ms, a, b); ms /= 5;
   cudaError_t e = cudaGetLastError();

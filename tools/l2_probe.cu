@@ -1,5 +1,5 @@
-// Micro-probe: how fast can 148 SMs gather random, L2-resident 1 KB rows (the SpMM access pattern)?
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a tools/l2_probe.cu -o /tmp/l2_probe && /tmp/l2_probe
+// Micro-probe: how fast can the 132 SMs of an H100 gather random, L2-resident 1 KB rows (the SpMM access pattern)?
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a tools/l2_probe.cu -o /tmp/l2_probe && /tmp/l2_probe
 // Prints GB/s for a table that fits L2 (64 MB), one that does not (1 GB), and a plain streaming read.
 #include <cstdio>
 #include <cstdint>
@@ -51,9 +51,9 @@ int main() {
       int* d; cudaMalloc(&d, n_idx * 4); cudaMemcpy(d, h, n_idx * 4, cudaMemcpyHostToDevice);
       for (int blocks_per_sm : {4, 8}) {
         cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-        gather_rows<<<148 * blocks_per_sm, 256>>>(X, d, n_idx, vec, sink);
+        gather_rows<<<132 * blocks_per_sm, 256>>>(X, d, n_idx, vec, sink);
         cudaEventRecord(a);
-        for (int it = 0; it < 5; ++it) gather_rows<<<148 * blocks_per_sm, 256>>>(X, d, n_idx, vec, sink);
+        for (int it = 0; it < 5; ++it) gather_rows<<<132 * blocks_per_sm, 256>>>(X, d, n_idx, vec, sink);
         cudaEventRecord(b); cudaEventSynchronize(b);
         float ms; cudaEventElapsedTime(&ms, a, b); ms /= 5;
         printf("{\"probe\":\"gather\",\"table_MB\":%zu,\"row_bytes\":%d,\"ctas_per_sm\":%d,\"GBps\":%.1f}\n", tb >> 20, rb,
@@ -62,9 +62,9 @@ int main() {
       cudaFree(d); delete[] h;
     }
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-    stream_read<<<148 * 8, 256>>>(X, tb / 16, sink);
+    stream_read<<<132 * 8, 256>>>(X, tb / 16, sink);
     cudaEventRecord(a);
-    for (int it = 0; it < 5; ++it) stream_read<<<148 * 8, 256>>>(X, tb / 16, sink);
+    for (int it = 0; it < 5; ++it) stream_read<<<132 * 8, 256>>>(X, tb / 16, sink);
     cudaEventRecord(b); cudaEventSynchronize(b);
     float ms; cudaEventElapsedTime(&ms, a, b); ms /= 5;
     printf("{\"probe\":\"stream\",\"table_MB\":%zu,\"GBps\":%.1f}\n", tb >> 20, (double)tb / ms / 1e6);

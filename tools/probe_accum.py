@@ -1,6 +1,11 @@
-"""Does the tcgen05 fp32 accumulator round to nearest or truncate?  Signed error of the 3xTF32 GEMMs against fp64 for
-(a) random-sign operands and (b) all-positive operands (a truncating accumulator shows up as a negative mean error
-that grows with the number of accumulation steps), next to torch.mm fp32 (cuBLAS) on the same inputs."""
+"""Does the tensor core's fp32 accumulate round to nearest or truncate, and what does that leave in the 3xTF32 kernels?
+
+(a) tf32_mm: cuBLAS with TF32 enabled (wgmma on Hopper) on operands already rounded to tf32, so every product is exact in
+    fp32 and the only error left is the accumulation.  With all-positive operands a round-to-nearest accumulator leaves a
+    mean signed error near zero; a truncating one leaves a negative mean that grows with K.
+(b) gemm / wgrad: signed error of this project's 3xTF32 kernels against fp64, random-sign and all-positive operands, next
+    to torch.mm fp32 (TF32 off) on the same inputs.
+One JSON line per case."""
 import json
 import sys
 from pathlib import Path
@@ -19,9 +24,22 @@ def stats(c, ref):
                 mean_signed_rel=float(er.mean()))
 
 
+def tf32(x):
+    return (x.view(torch.int32) + 0x1000 & -0x2000).view(torch.float32)      # round to nearest tf32, as the kernels do
+
+
 def main():
     torch.manual_seed(0)
     dev = "cuda"
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    print(json.dumps(dict(device=torch.cuda.get_device_name(0), sms=sms)), flush=True)
+    for K in (256, 4096, 65536):
+        a, b = tf32(torch.rand(1024, K, device=dev)), tf32(torch.rand(256, K, device=dev))
+        ref = a.double() @ b.double().t()
+        torch.backends.cuda.matmul.allow_tf32 = True
+        c = a @ b.t()
+        torch.backends.cuda.matmul.allow_tf32 = False
+        print(json.dumps(dict(op="tf32_mm", positive=True, K=K, cublas_tf32=stats(c, ref))), flush=True)
     for positive in (False, True):
         for K in (32, 128, 256, 1024):
             M, N = 4096, 256
@@ -33,15 +51,15 @@ def main():
             c = ops.gemm_tf32x3(a, hi, lo)
             c32 = a @ b.t()
             print(json.dumps(dict(op="gemm", positive=positive, K=K, tf32x3=stats(c, ref), cublas_fp32=stats(c32, ref))), flush=True)
-        for rows in (148 * 16, 148 * 16 * 8, 148 * 16 * 72):
+        for rows in (sms * 16, sms * 16 * 8, sms * 16 * 72):
             x = torch.randn(rows, 256, device=dev); g = torch.randn(rows, 256, device=dev)
             if positive:
                 x, g = x.abs(), g.abs()
             ref = x.double().t() @ g.double()
             w = ops.gemm_wgrad_tf32x3(x, g)
             w32 = x.t() @ g
-            print(json.dumps(dict(op="wgrad", positive=positive, rows=rows, chain_mmas=rows // 148 // 8 * 3, tf32x3=stats(w, ref),
-                                  cublas_fp32=stats(w32, ref))), flush=True)
+            print(json.dumps(dict(op="wgrad", positive=positive, rows=rows, tf32x3=stats(w, ref), cublas_fp32=stats(w32, ref))),
+                  flush=True)
 
 
 if __name__ == "__main__":

@@ -18,7 +18,7 @@ if sys.argv[1] == "gemm":
         ops.gemm_tf32x3(x, hi, lo, out=out)
 else:
     g = torch.randn(M, N, device="cuda")
-    out, ws = torch.empty(K, N, device="cuda"), torch.empty(148 * K * N, device="cuda")
+    out, ws = torch.empty(K, N, device="cuda"), torch.empty(ops.wgrad_workspace_floats(K, N), device="cuda")
     for _ in range(4):
         ops.gemm_wgrad_tf32x3(x, g, out=out, workspace=ws)
 torch.cuda.synchronize()
