@@ -23,6 +23,16 @@ inline int check_launch() {
 
 constexpr unsigned FULL_MASK = 0xffffffffu;
 
+// One element of torch.optim.Adam (no amsgrad, no weight decay); step_size = lr / (1 - b1^t), inv_sqrt_bc2 = rsqrt(1 - b2^t).
+// Shared by the flat-buffer Adam and the embedding-table Adam, which must agree bit for bit.
+__device__ __forceinline__ void adam_update(float& p, float& m, float& v, float g, float b1, float b2, float eps,
+                                            float step_size, float inv_sqrt_bc2) {
+  const float mi = b1 * m + (1.f - b1) * g;
+  const float vi = b2 * v + (1.f - b2) * g * g;
+  m = mi; v = vi;
+  p -= step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
+}
+
 // ---- small vector algebra so kernels can be written once over float/float2/float4
 template <typename V> struct VecTraits;
 template <> struct VecTraits<float> { static constexpr int W = 1; };

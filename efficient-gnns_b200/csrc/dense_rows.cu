@@ -275,6 +275,19 @@ static inline bool dropout_p16(float p, uint32_t& thr16) {
   return p > 0.f && t == (double)thr16;
 }
 
+// ---------------------------------------------------------------- backward of ReLU+dropout (no BatchNorm)
+// dY = dOut * [Xout > 0] / (1-p)   (the R-GCN's hidden layers: relu -> dropout straight after the conv)
+__global__ void __launch_bounds__(256) relu_dropout_bwd_kernel(const float4* __restrict__ dOut, const float4* __restrict__ Xout,
+                                                               float4* dY, int64_t n_vec, float inv_keep) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 g = dOut[i], x = Xout[i];
+    float4 d;
+    d.x = x.x > 0.f ? g.x * inv_keep : 0.f; d.y = x.y > 0.f ? g.y * inv_keep : 0.f;
+    d.z = x.z > 0.f ? g.z * inv_keep : 0.f; d.w = x.w > 0.f ? g.w * inv_keep : 0.f;
+    dY[i] = d;
+  }
+}
+
 // ---------------------------------------------------------------- backward of BN(train)+ReLU+dropout
 // dz = dOut * [Xout > 0] / (1-p)       (Xout>0  <=>  kept by dropout AND relu-active)
 // pass 1: partial column sums of dz and dz*xhat, xhat = (Y-mean)*invstd
@@ -385,13 +398,8 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   const float t = (float)(*step + 1);
   const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
   const float step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float gi = g[i];
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi; v[i] = vi;
-    p[i] -= step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
-  }
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    adam_update(p[i], m[i], v[i], g[i], b1, b2, eps, step_size, inv_sqrt_bc2);
 }
 __global__ void adam_tick_kernel(int32_t* step) { *step += 1; }
 
@@ -526,6 +534,18 @@ extern "C" int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K,
   uint32_t thr16 = 0;
   const int p16 = dropout_p16(p, thr16) ? 1 : 0;
   dropout_mask_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(mask, n_vec, p, p16, thr16, seed, offset);
+  return check_launch();
+}
+
+extern "C" int b200gnn_relu_dropout_bwd_f32(const float* dOut, const float* Xout, float* dY, int64_t n_rows, int64_t K,
+                                            float p, void* stream) {
+  if (!rows_ok(n_rows, K) || p < 0.f || p >= 1.f) return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  if (!dOut || !Xout || !dY || !aligned_to(dOut, 16) || !aligned_to(Xout, 16) || !aligned_to(dY, 16)) return B200GNN_ERR_BAD_ARG;
+  const int64_t n_vec = n_rows * (K / 4);
+  const float inv_keep = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  relu_dropout_bwd_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const float4*>(dOut), reinterpret_cast<const float4*>(Xout), reinterpret_cast<float4*>(dY), n_vec, inv_keep);
   return check_launch();
 }
 

@@ -1,7 +1,8 @@
 // Weight-gradient GEMM on the Hopper tensor cores:   dW[Kin, Nout] = X[Nn, Kin]^T · G[Nn, Nout]   (fp32-faithful, 3xTF32)
 //
 // The contraction runs over the NODE index (Nn ~ 1.7e5) and the result is tiny (<= 256 x 256), so this is a
-// split-K problem: the output is cut into 128 x 128 tiles, every CTA owns one tile and a contiguous range of nodes,
+// split-K problem: the output is cut into 128 x 128 tiles (Kin and Nout are padded up to the tile grid by TMA zero fill;
+// the padding rows and columns of the partials are dropped by the reduction), every CTA owns one tile and a contiguous range of nodes,
 // streams its slices of X and G through shared memory exactly once, keeps the tile's partial in registers, and a small
 // second kernel adds the per-range partials in a fixed order (deterministic, no atomics).
 //
@@ -29,11 +30,15 @@ constexpr int OP_BYTES = 128 * BKN * 4;          // 16 KB: one transposed operan
 constexpr int T_BYTES = 4 * OP_BYTES;            // X_hi, X_lo, G_hi, G_lo
 constexpr int SMEM_BYTES = STAGES * RAW_BYTES + 2 * T_BYTES + 256 + 1024;
 constexpr int MAX_RANGES = 132;                  // node ranges (workspace partials): one CTA per SM over all tiles
+// The workspace holds at most the partials of the largest shape of the 128/256-wide layers (132 ranges of 256 x 256);
+// wider outputs have more tiles, fill the SMs with fewer ranges and get proportionally fewer partial slots.
+constexpr int64_t MAX_PARTIAL_FLOATS = (int64_t)MAX_RANGES * 256 * 256;
+constexpr int MAX_KIN = 2048, MAX_NOUT = 512;
 static_assert(SMEM_BYTES <= 232448, "shared memory");
 
 struct Params {
-  float* partial;   // [n_ranges][Kin][Npad],  Npad = Nout rounded up to 32 (TMA zero-fills the missing columns)
-  int32_t Nn, Kin, Nout, Npad, num_kb;
+  float* partial;   // [n_ranges][Kpad][Npad], Kpad = Kin rounded up to 128, Npad = Nout rounded up to 32 (TMA zero fill)
+  int32_t Nn, Kin, Kpad, Nout, Npad, num_kb;
   int32_t n_tn, n_ranges;   // column tiles of dW, node ranges
 };
 
@@ -45,7 +50,7 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   uint64_t* full = reinterpret_cast<uint64_t*>(tbuf + 2 * T_BYTES);
   uint64_t* empty = full + STAGES;
 
-  const int tiles = (p.Kin / TM) * p.n_tn;
+  const int tiles = (p.Kpad / TM) * p.n_tn;
   const int tile = (int)blockIdx.x % tiles, range = (int)blockIdx.x / tiles;
   const int mt = tile / p.n_tn, nt = tile % p.n_tn;
   const int kb0 = (int)((int64_t)p.num_kb * range / p.n_ranges);
@@ -137,7 +142,7 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
     for (int j = 0; j < 64; ++j) sum[j] += acc[j];
   }
   // fragment -> partial: rows mt*128 + 64 cw + 16 (warp % 4) + lane/4 (+8), columns nt*128 + 8 j + 2 (lane % 4)
-  float* out = p.partial + (size_t)range * p.Kin * p.Npad;
+  float* out = p.partial + (size_t)range * p.Kpad * p.Npad;
   const int row0 = mt * TM + cw * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
@@ -149,15 +154,15 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   }
 }
 
-// dW[r][c] = sum over CTAs of partial[cta][r][c], dropping the padding columns.  32 float4 columns x 8 groups per
+// dW[r][c] = sum over CTAs of partial[cta][r][c], dropping the padding rows and columns.  32 float4 columns x 8 groups per
 // CTA: group g adds partials g, g+8, ... and the groups are combined in order through shared memory (fixed order,
 // deterministic; 8x shorter dependent chains than one thread per element).
 constexpr int RED_VECS = 32, RED_GROUPS = 8;
 __global__ void __launch_bounds__(RED_VECS * RED_GROUPS) wgrad_reduce_kernel(const float4* __restrict__ partial, int n_part,
-                                                                             int Kin, int Nout, int Npad,
+                                                                             int Kin, int Kpad, int Nout, int Npad,
                                                                              float* __restrict__ out) {
   __shared__ float4 sh[RED_GROUPS][RED_VECS];
-  const int64_t n_vec = (int64_t)Kin * Npad / 4;
+  const int64_t n_vec = (int64_t)Kpad * Npad / 4;
   const int v = threadIdx.x % RED_VECS, g = threadIdx.x / RED_VECS;
   const int64_t i = (int64_t)blockIdx.x * RED_VECS + v;
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -170,7 +175,7 @@ __global__ void __launch_bounds__(RED_VECS * RED_GROUPS) wgrad_reduce_kernel(con
   __syncthreads();
   if (g != 0 || i >= n_vec) return;
   const int row = (int)(i / (Npad / 4)), c4 = (int)(i % (Npad / 4)) * 4;
-  if (c4 >= Nout) return;
+  if (c4 >= Nout || row >= Kin) return;
 #pragma unroll
   for (int j = 1; j < RED_GROUPS; ++j) {
     const float4 x = sh[j][v];
@@ -192,6 +197,14 @@ static bool make_map_rows(CUtensorMap* m, const float* base, int64_t rows, int64
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+static int64_t pad_k(int64_t Kin) { return (Kin + TM - 1) / TM * TM; }
+static int64_t pad_n(int64_t Nout) { return (Nout + 31) / 32 * 32; }
+// node ranges the workspace has room for: MAX_RANGES for every output up to 256 x 256
+static int range_cap(int64_t Kin, int64_t Nout) {
+  const int64_t c = MAX_PARTIAL_FLOATS / (pad_k(Kin) * pad_n(Nout));
+  return (int)(c > MAX_RANGES ? MAX_RANGES : (c < 1 ? 1 : c));
+}
+
 }  // namespace wgrad
 }  // namespace b200gnn
 
@@ -199,15 +212,17 @@ using namespace b200gnn;
 
 extern "C" int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout) {
   if (Kin <= 0 || Nout <= 0) return B200GNN_ERR_BAD_ARG;
-  return wgrad::MAX_RANGES * Kin * ((Nout + 31) / 32 * 32);
+  if (Kin > wgrad::MAX_KIN || Nout > wgrad::MAX_NOUT) return B200GNN_ERR_UNSUPPORTED;
+  return wgrad::range_cap(Kin, Nout) * wgrad::pad_k(Kin) * wgrad::pad_n(Nout);
 }
 
 extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW,
                                              int64_t Nn, int64_t Kin, int64_t Nout, float* workspace, void* stream) {
   if (!X || !G || !dW || !workspace || Nn <= 0 || Kin <= 0 || Nout <= 0 || ldx < Kin || ldg < Nout || Nn >= INT32_MAX)
     return B200GNN_ERR_BAD_ARG;
-  // tensor-core tiling: Kin in {128, 256}; Nout a multiple of 4 up to 256 (padded to 32 by TMA zero fill); alignment
-  if (Kin % 128 || Kin > 256 || Nout % 4 || Nout > 256 || ldx % 4 || ldg % 4 || !aligned_to(X, 16) || !aligned_to(G, 16) ||
+  // tensor-core tiling: Kin a multiple of 4 up to 2048 (padded to 128), Nout a multiple of 4 up to 512 (padded to 32), both
+  // by TMA zero fill; 16-byte alignment
+  if (Kin % 4 || Kin > wgrad::MAX_KIN || Nout % 4 || Nout > wgrad::MAX_NOUT || ldx % 4 || ldg % 4 || !aligned_to(X, 16) || !aligned_to(G, 16) ||
       !aligned_to(dW, 16) || !aligned_to(workspace, 16))
     return B200GNN_ERR_UNSUPPORTED;
   CUtensorMap tX, tG;
@@ -225,20 +240,22 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const 
   cudaStream_t st = (cudaStream_t)stream;
   wgrad::Params p;
   p.partial = workspace; p.Nn = (int32_t)Nn; p.Kin = (int32_t)Kin; p.Nout = (int32_t)Nout;
-  p.Npad = (int32_t)((Nout + 31) / 32 * 32);
+  p.Kpad = (int32_t)wgrad::pad_k(Kin);
+  p.Npad = (int32_t)wgrad::pad_n(Nout);
   p.num_kb = (int32_t)((Nn + wgrad::BKN - 1) / wgrad::BKN);
   p.n_tn = (p.Npad + wgrad::TN - 1) / wgrad::TN;
-  const int tiles = (int)(Kin / wgrad::TM) * p.n_tn;
+  const int tiles = (int)(p.Kpad / wgrad::TM) * p.n_tn;
   int ranges = sms / tiles;                          // one CTA per SM over all tiles
-  if (ranges > wgrad::MAX_RANGES) ranges = wgrad::MAX_RANGES;   // the workspace holds MAX_RANGES partials
+  const int cap = wgrad::range_cap(Kin, Nout);       // the workspace holds this many partials
+  if (ranges > cap) ranges = cap;
   if (ranges > p.num_kb) ranges = p.num_kb;
   if (ranges < 1) ranges = 1;
   p.n_ranges = ranges;
   int rc;
   wgrad::wgrad_tf32x3_kernel<<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
   if ((rc = check_launch())) return rc;
-  const int64_t n_vec = Kin * (int64_t)p.Npad / 4;
+  const int64_t n_vec = (int64_t)p.Kpad * p.Npad / 4;
   wgrad::wgrad_reduce_kernel<<<(int)((n_vec + wgrad::RED_VECS - 1) / wgrad::RED_VECS), wgrad::RED_VECS * wgrad::RED_GROUPS, 0, st>>>(
-      reinterpret_cast<const float4*>(workspace), ranges, (int)Kin, (int)Nout, p.Npad, dW);
+      reinterpret_cast<const float4*>(workspace), ranges, (int)Kin, p.Kpad, (int)Nout, p.Npad, dW);
   return check_launch();
 }

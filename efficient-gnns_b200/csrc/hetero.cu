@@ -62,6 +62,54 @@ __global__ void __launch_bounds__(256) typed_scatter_kernel(const float* __restr
   }
 }
 
+// Embedding Adam without a dense gradient.  Pass 1 marks the rows of the table the batch touches: head[j] = position in
+// `order` of the first node of the run with key (table_type, j).  Pass 2 sweeps the whole table, one warp per row: the
+// row's gradient is its run summed exactly as typed_scatter_kernel sums it (0 for rows outside the batch), followed by
+// the Adam element update of adam_kernel, and head[j] is reset to -1 for the next call.
+__global__ void __launch_bounds__(256) embedding_heads_kernel(const int64_t* __restrict__ node_type,
+                                                              const int64_t* __restrict__ local_idx,
+                                                              const int64_t* __restrict__ order, int64_t n, int64_t table_type,
+                                                              int64_t rows, int32_t* __restrict__ head) {
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = order[p];
+    if (p > 0 && same_key(node_type, local_idx, i, order[p - 1])) continue;
+    const int64_t j = local_idx[i];
+    if (node_type[i] == table_type && j >= 0 && j < rows) head[j] = (int32_t)p;
+  }
+}
+
+__global__ void __launch_bounds__(256) embedding_adam_kernel(const float* __restrict__ d_out, int64_t ldd,
+                                                             const int64_t* __restrict__ node_type,
+                                                             const int64_t* __restrict__ local_idx,
+                                                             const int64_t* __restrict__ order, int64_t n, int F,
+                                                             float* __restrict__ table, float* __restrict__ exp_avg,
+                                                             float* __restrict__ exp_avg_sq, int64_t rows, int32_t* head,
+                                                             float lr, float b1, float b2, float eps,
+                                                             const int32_t* __restrict__ step) {
+  const float t = (float)(*step + 1);
+  const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
+  const float step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5), nwarps = (int64_t)gridDim.x * 8;
+  for (int64_t j = warp; j < rows; j += nwarps) {
+    const int32_t p = head[j];
+    __syncwarp();
+    if (p >= 0 && lane == 0) head[j] = -1;
+    const int64_t i = p >= 0 ? order[p] : 0;
+    const size_t o = (size_t)j * F;
+    for (int k = lane; k < F; k += 32) {
+      float g = 0.f;
+      if (p >= 0)
+        for (int64_t q = p; q < n; ++q) {
+          const int64_t r = order[q];
+          if (q > p && !same_key(node_type, local_idx, r, i)) break;
+          g += d_out[(size_t)r * ldd + k];
+        }
+      adam_update(table[o + k], exp_avg[o + k], exp_avg_sq[o + k], g, b1, b2, eps, step_size, inv_sqrt_bc2);
+    }
+  }
+}
+
 static inline int rows_grid(int64_t n) {
   int64_t g = (n + 7) / 8;
   if (g > 132 * 16) g = 132 * 16;
@@ -105,5 +153,26 @@ extern "C" int b200gnn_typed_scatter_f32(const float* d_out, int64_t ldd, const 
   if (n == 0) return B200GNN_OK;
   if (!d_out || !node_type || !local_idx || !order) return B200GNN_ERR_BAD_ARG;
   typed_scatter_kernel<<<rows_grid(n), 256, 0, (cudaStream_t)stream>>>(d_out, ldd, node_type, local_idx, order, n, (int)F, T);
+  return check_launch();
+}
+
+extern "C" int b200gnn_embedding_adam_f32(const float* d_out, int64_t ldd, const int64_t* node_type, const int64_t* local_idx,
+                                          const int64_t* order, int64_t n, int64_t table_type, float* table, float* exp_avg,
+                                          float* exp_avg_sq, int64_t rows, int64_t F, int32_t* head, float lr, float beta1,
+                                          float beta2, float eps, const int32_t* step, void* stream) {
+  if (n < 0 || rows < 0 || rows >= INT32_MAX || n >= INT32_MAX || F <= 0 || F > (1 << 20) || ldd < F || !step)
+    return B200GNN_ERR_BAD_ARG;
+  if (rows == 0) return B200GNN_OK;
+  if (!table || !exp_avg || !exp_avg_sq || !head || (n > 0 && (!d_out || !node_type || !local_idx || !order)))
+    return B200GNN_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (n > 0) {
+    int64_t g = (n + 255) / 256;
+    embedding_heads_kernel<<<(int)(g > 132 * 8 ? 132 * 8 : g), 256, 0, st>>>(node_type, local_idx, order, n, table_type, rows, head);
+    if ((rc = check_launch())) return rc;
+  }
+  embedding_adam_kernel<<<rows_grid(rows), 256, 0, st>>>(d_out, ldd, node_type, local_idx, order, n, (int)F, table, exp_avg,
+                                                         exp_avg_sq, rows, head, lr, beta1, beta2, eps, step);
   return check_launch();
 }

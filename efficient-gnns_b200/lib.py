@@ -56,6 +56,7 @@ SIGNATURES = {
     "b200gnn_affine_relu_dropout_scatter_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32p, _f32p, _int, _f32, _u64, _u64,
                                                        _i32p, _u64, _i32p, _u64, _i64, _i64, _ptr, _ptr, _i32, _i64, _ptr]),
     "b200gnn_dropout_mask_u8": (_int, [_ptr, _i64, _i64, _f32, _u64, _u64, _ptr]),
+    "b200gnn_relu_dropout_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _ptr]),
     "b200gnn_bn_act_bwd_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32, _f32p, _f32p,
                                       _f32p, _f32p, _f32p, _i64, _f32p, _ptr]),
     "b200gnn_bn_act_bwd_reduce_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32, _f32p, _i64, _ptr]),
@@ -112,6 +113,8 @@ SIGNATURES = {
     "b200gnn_graph_coalesce_i64": (_int, [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _i32p, _ptr, _ptr, _ptr, _ptr]),
     "b200gnn_typed_gather_f32": (_int, [_ptr, _ptr, _i32, _ptr, _ptr, _i64, _i64, _f32p, _i64, _i32p, _ptr]),
     "b200gnn_typed_scatter_f32": (_int, [_f32p, _i64, _ptr, _ptr, _ptr, _i64, _i64, _ptr, _ptr, _i32, _ptr]),
+    "b200gnn_embedding_adam_f32": (_int, [_f32p, _i64, _ptr, _ptr, _ptr, _i64, _i64, _f32p, _f32p, _f32p, _i64, _i64, _i32p,
+                                          _f32, _f32, _f32, _f32, _i32p, _ptr]),
     "b200gnn_arena_alloc": (_int, [_i64, C.POINTER(C.c_void_p)]),
     "b200gnn_arena_free": (_int, [_ptr]),
     "b200gnn_ipc_get_handle": (_int, [_ptr, _ptr]),

@@ -357,6 +357,7 @@ def gemm_tf32x3_bcast(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, d
 
 
 def wgrad_supported(k_in: int, n_out: int) -> bool:
+    """Shapes gemm_wgrad_tf32x3 accepts by default: the 128/256-row tilings of the GCN / SAGE layers."""
     return k_in in (128, 256) and n_out % 4 == 0 and 0 < n_out <= 256
 
 
@@ -366,16 +367,27 @@ def wgrad_workspace_floats(k_in: int, n_out: int) -> int:
 
 
 def gemm_wgrad_tf32x3(x: torch.Tensor, g: torch.Tensor, out: Optional[torch.Tensor] = None,
-                      workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[Kin,Nout] = x[Nn,Kin]^T @ g[Nn,Nout] on the tensor cores with fp32 fidelity (split-K over nodes)."""
+                      workspace: Optional[torch.Tensor] = None, wide: bool = False) -> torch.Tensor:
+    """out[Kin,Nout] = x[Nn,Kin]^T @ g[Nn,Nout] on the tensor cores with fp32 fidelity (split-K over nodes).
+
+    By default only the shapes of ``wgrad_supported`` are accepted (others raise B200GnnError), so a caller that picks its
+    path by that predicate never reaches a padded tiling by accident.  ``wide=True`` accepts everything the kernel takes:
+    Kin and Nout multiples of 4 up to 2048 and 512, ragged 128-row / 32-column tiles zero-filled (the R-GCN's
+    [Wroot | W_r1 | ...] blocks)."""
     nn_, k_in = x.shape
     n_out = g.shape[1]
     assert g.shape[0] == nn_
+    if not wide and not wgrad_supported(k_in, n_out):
+        raise lib.B200GnnError(f"gemm_wgrad_tf32x3: Kin={k_in}, Nout={n_out} is outside the 128/256-row tilings "
+                               "(pass wide=True for the padded ones)")
     L = lib.load()
     if out is None:
         out = torch.empty(k_in, n_out, dtype=torch.float32, device=x.device)
     if workspace is None:
-        workspace = torch.empty(int(L.b200gnn_wgrad_workspace_floats(k_in, n_out)), dtype=torch.float32, device=x.device)
+        n_ws = int(L.b200gnn_wgrad_workspace_floats(k_in, n_out))
+        if n_ws < 0:
+            lib.check(n_ws, "wgrad_workspace_floats")
+        workspace = torch.empty(n_ws, dtype=torch.float32, device=x.device)
     lib.check(L.b200gnn_gemm_wgrad_tf32x3_f32(_f32(x, "x"), x.stride(0), _f32(g, "g"), g.stride(0), _f32(out, "out"), nn_,
                                               k_in, n_out, _f32(workspace, "workspace"), lib.stream_ptr()),
               "gemm_wgrad_tf32x3_f32")
@@ -411,3 +423,61 @@ def bn_act_bwd_apply(d_out, x_out, y, mean, invstd, gamma, sums, n_norm: int, p:
         _f32(gamma, "gamma"), _f32(sums, "sums"), sum_slots, n_norm, n, K, p, _f32(d_y, "d_y"), _f32(d_gamma, "d_gamma"),
         _f32(d_beta, "d_beta"), _f32(d_bias, "d_bias"), _f32(partial, "partial"), partial.shape[0], _f32(coef, "coef"),
         lib.stream_ptr()), "bn_act_bwd_apply_f32")
+
+
+# ----------------------------------------------------------------------------- R-GCN training passes
+def relu_dropout_bwd(d_out: torch.Tensor, x_out: torch.Tensor, p: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Backward of x_out = dropout_p(relu(y)): d_y = d_out * [x_out > 0] / (1-p) (contiguous [n, K]; out may be d_out)."""
+    n, K = x_out.shape
+    assert d_out.shape == x_out.shape and d_out.is_contiguous() and x_out.is_contiguous()
+    out = torch.empty_like(x_out) if out is None else out
+    lib.check(lib.load().b200gnn_relu_dropout_bwd_f32(_f32(d_out, "d_out"), _f32(x_out, "x_out"), _f32(out, "out"), n, K, float(p),
+                                                      lib.stream_ptr()), "relu_dropout_bwd_f32")
+    return out
+
+
+def _table_arrays(tables: dict, n_tables: int):
+    import ctypes as C
+    ptrs = (C.c_void_p * n_tables)()
+    rows = (C.c_int64 * n_tables)()
+    for k, t in tables.items():
+        ptrs[k], rows[k] = t.data_ptr(), t.shape[0]
+    return ptrs, rows
+
+
+def typed_gather(tables: dict, n_tables: int, node_type: torch.Tensor, local_idx: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out[i] = tables[node_type[i]][local_idx[i]] (zero rows for types without a table); tables: {type: [rows, F] fp32}."""
+    ptrs, rows = _table_arrays(tables, n_tables)
+    err = torch.zeros(1, dtype=torch.int32, device=out.device)
+    lib.check(lib.load().b200gnn_typed_gather_f32(ptrs, rows, n_tables, lib.dptr(node_type, torch.int64, "node_type"),
+                                                  lib.dptr(local_idx, torch.int64, "local_idx"), out.shape[0], out.shape[1],
+                                                  _f32(out, "out"), out.stride(0), err.data_ptr(), lib.stream_ptr()),
+              "typed_gather_f32")
+    return out
+
+
+def typed_scatter(d_out: torch.Tensor, node_type: torch.Tensor, local_idx: torch.Tensor, order: torch.Tensor, grads: dict,
+                  n_tables: int) -> None:
+    """grads[t][j] = sum of d_out[i] over nodes (node_type, local_idx) == (t, j), added in ``order`` (rows outside the batch are
+    left untouched: pass zeroed tables for a dense gradient)."""
+    ptrs, rows = _table_arrays(grads, n_tables)
+    lib.check(lib.load().b200gnn_typed_scatter_f32(_f32(d_out, "d_out"), d_out.stride(0), lib.dptr(node_type, torch.int64, "node_type"),
+                                                   lib.dptr(local_idx, torch.int64, "local_idx"), lib.dptr(order, torch.int64, "order"),
+                                                   d_out.shape[0], d_out.shape[1], ptrs, rows, n_tables, lib.stream_ptr()),
+              "typed_scatter_f32")
+
+
+def embedding_adam(d_out: torch.Tensor, node_type: torch.Tensor, local_idx: torch.Tensor, order: torch.Tensor, table_type: int,
+                   table: torch.Tensor, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, head: torch.Tensor, step: torch.Tensor,
+                   lr: float, betas=(0.9, 0.999), eps: float = 1e-8) -> None:
+    """Adam over one embedding table whose gradient is typed_scatter(d_out) (``order``: the rows of d_out sorted by
+    (node_type, local_idx)); bit-identical to the scatter into a zeroed dense gradient + adam_step, reads ``step`` without
+    advancing it.  head: int32 [rows] scratch, all -1 (restored on return)."""
+    rows, F_ = table.shape
+    assert exp_avg.shape == table.shape == exp_avg_sq.shape and head.numel() >= rows and d_out.shape[1] == F_
+    lib.check(lib.load().b200gnn_embedding_adam_f32(
+        _f32(d_out, "d_out"), d_out.stride(0), lib.dptr(node_type, torch.int64, "node_type"),
+        lib.dptr(local_idx, torch.int64, "local_idx"), lib.dptr(order, torch.int64, "order"), d_out.shape[0], int(table_type),
+        _f32(table, "table"), _f32(exp_avg, "exp_avg"), _f32(exp_avg_sq, "exp_avg_sq"), rows, F_,
+        lib.dptr(head, torch.int32, "head"), lr, betas[0], betas[1], eps, lib.dptr(step, torch.int32, "step"), lib.stream_ptr()),
+        "embedding_adam_f32")

@@ -187,6 +187,10 @@ int b200gnn_affine_relu_dropout_scatter_f32(const float* Y, float* out, int64_t 
                                             const int32_t* row_off, int32_t world, int64_t ld_dst, void* stream);
 int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K, float p,
                             uint64_t seed, uint64_t offset, void* stream);
+/* Backward of out = dropout_p(relu(Y)) (no BatchNorm): dY = dOut * [Xout > 0] / (1-p), contiguous [n_rows, K]
+ * rows, K a multiple of 4; dY may alias dOut. */
+int b200gnn_relu_dropout_bwd_f32(const float* dOut, const float* Xout, float* dY,
+                                 int64_t n_rows, int64_t K, float p, void* stream);
 /* Backward of out = dropout_p(relu(BN_train(Y))): given dOut, out (for the
  * mask: out>0 <=> kept and active), Y and the saved batch mean/invstd, writes
  * dY, dgamma[K], dbeta[K] and (if non-NULL) dbias[K] = column sums of dY.
@@ -307,8 +311,9 @@ int b200gnn_gemm_tf32x3_bcast_f32(const float* A, int64_t lda, const float* B_hi
 
 /* Weight gradient  dW[Kin,Nout] = X[Nn,Kin]^T * G[Nn,Nout]  (GCNConv weight.grad / nn.Linear weight.grad^T),
  * split-K over the node index on the Hopper tensor cores (wgmma, 3xTF32), partials reduced in fixed order.
- * Kin in {128,256}, Nout a multiple of 4 up to 256 (else B200GNN_ERR_UNSUPPORTED: caller keeps the library GEMM).
- * workspace: float[b200gnn_wgrad_workspace_floats(Kin,Nout)]. */
+ * Kin a multiple of 4 up to 2048, Nout a multiple of 4 up to 512 (else B200GNN_ERR_UNSUPPORTED); ragged edges are
+ * zero-filled by TMA.  workspace: float[b200gnn_wgrad_workspace_floats(Kin,Nout)]: at most 132 node-range partials of the
+ * padded [Kin, Nout] tile grid, fewer for outputs larger than 256 x 256. */
 int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout);
 int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G,
                                   int64_t ldg, float* dW, int64_t Nn,
@@ -488,6 +493,18 @@ int b200gnn_peer_exchange_f32(const b200gnn_copy2d* copies, int32_t n, int64_t w
 int b200gnn_typed_gather_f32(const float* const* tables, const int64_t* table_rows, int32_t n_tables,
                              const int64_t* node_type, const int64_t* local_idx, int64_t n, int64_t F,
                              float* out, int64_t ldo, int32_t* error_flag, void* stream);
+/* Adam over ONE embedding table (rows x F; the table of node type table_type) whose gradient is the typed_scatter of
+ * d_out: row j's gradient is the sum of the d_out rows of the nodes with (node_type, local_idx) == (table_type, j), added in
+ * `order`, or 0 if there is none, and every row of the table gets the b200gnn_adam_step_f32 update.  Bit-identical to
+ * b200gnn_typed_scatter_f32 into a zeroed table followed by b200gnn_adam_step_f32, without the dense gradient.
+ * order: the n nodes sorted by (node_type, local_idx).  head: int32[rows] scratch, all -1 on entry, restored on return.
+ * *step is read (steps already taken) and NOT incremented: the flat-buffer b200gnn_adam_step_f32 that runs after it
+ * owns the counter. */
+int b200gnn_embedding_adam_f32(const float* d_out, int64_t ldd, const int64_t* node_type,
+                               const int64_t* local_idx, const int64_t* order, int64_t n,
+                               int64_t table_type, float* table, float* exp_avg, float* exp_avg_sq,
+                               int64_t rows, int64_t F, int32_t* head, float lr, float beta1,
+                               float beta2, float eps, const int32_t* step, void* stream);
 int b200gnn_typed_scatter_f32(const float* d_out, int64_t ldd, const int64_t* node_type,
                               const int64_t* local_idx, const int64_t* order, int64_t n, int64_t F,
                               float* const* d_tables, const int64_t* table_rows, int32_t n_tables,
