@@ -9,12 +9,15 @@
 //                                                    x_lo = (x - x_hi) rounded to tf32,
 // three wgmma.mma_async ... .tf32 instructions per K-step.  The dropped terms are O(2^-22) relative.  B (the small
 // weight matrix) arrives pre-split from b200gnn_split_tf32_f32; A (the big activation matrix) is split on the fly in
-// shared memory, so HBM only ever sees one fp32 copy of it.
+// registers, so HBM only ever sees one fp32 copy of it.
 //
 // Structure (one persistent CTA per SM, 384 threads = 3 warpgroups):
 //   warpgroup 0     TMA producer: one thread, cp.async.bulk.tensor 128x32 fp32 boxes (128B swizzle) of A, B_hi, B_lo
-//   warpgroups 1-2  consumers, 64 rows of the 128-row tile each: split their rows of the A tile in place into
-//                   (A_hi, A_lo) while the previous stage's wgmmas run, issue 12 wgmmas per stage, then the epilogue.
+//   warpgroups 1-2  consumers, 64 rows of the 128-row tile each: every thread loads its wgmma A fragment of the stage
+//                   from the A tile and splits it into (hi, lo) registers while the previous stage's wgmmas run, issues
+//                   12 wgmmas per stage (A from registers, B from shared memory), then the epilogue.  A_hi / A_lo never
+//                   go through shared memory, which keeps a stage's shared-memory traffic (TMA writes, the fragment
+//                   loads, the B reads of the wgmmas) under its tensor-core time.
 // Accumulation: the tensor core's fp32 accumulate truncates instead of rounding to nearest (tools/probe_accum.py), and its
 // error grows with the number of updates of one accumulator.  Each stage's 12 wgmmas therefore go to a fresh register accumulator that is
 // then added (fp32, round to nearest) into the tile's running sum: no tensor-core chain is longer than one stage.
@@ -31,7 +34,6 @@ constexpr int BM = 128, BK = 32;
 constexpr int THREADS = 384;
 constexpr int CONSUMER_WARPS = 8;                       // warp q owns rows [16 q, 16 q + 16) of the tile
 constexpr int TILE_BYTES = BM * BK * 4;                 // 16 KB: one 128 x 32 fp32 A tile
-constexpr int WG_TILE_BYTES = TILE_BYTES / 2;           // the 64 rows of one consumer warpgroup
 constexpr int BAR_BYTES = 256;
 constexpr int EPI_BYTES = CONSUMER_WARPS * 16 * 32 * 4; // one 16x32 staging block per consumer warp (16-byte chunks swizzled)
 constexpr int STAT_MAX_N = 256;                         // fused column statistics: output width limit
@@ -40,19 +42,20 @@ constexpr int XY_ROWS = 16;
 constexpr int XY_SLOT_BYTES = 2 * XY_ROWS * 32 * 4;     // one 16x32 fp32 block of Xout + the same block of Y
 constexpr int XY_BYTES = CONSUMER_WARPS * 2 * XY_SLOT_BYTES;  // 8 consumer warps x 2 slots (stat_mode 2 with TMA-staged operands)
 constexpr int XY_BAR_OFF = 128;                         // byte offset of the 16 Xout/Y mbarriers inside the barrier block
-// BatchNorm-backward epilogue: the TMA-staged Xout / Y path pays for its 64 KB with one mainloop stage, which only narrow-K
-// launches (epilogue-bound) win back; measured on H100 (BENCH.md): K=40 TMA ahead, K=256 the register path ahead.
+// BatchNorm-backward epilogue: the TMA-staged Xout / Y path pays for its 64 KB with two of the four mainloop stages, which
+// only narrow-K launches (epilogue-bound) win back; measured on H100 (BENCH.md): K=40 TMA ahead, K=256 the register path ahead.
 constexpr int BNBWD_TMA_MAX_K = 128;
 
 // Tile shape: BN_T output columns per tile (the wgmma N) and the number of smem stages that fit.
-//   Wide  <128, 3>: 3 x 64 KB stages.
-//   Narrow <48, 4>: for N <= 48 (the 40-class logits): the B tiles shrink to 6 KB, one more stage fits (the narrow
+//   Wide  <128, 4>: 4 x 48 KB stages.
+//   Narrow <48, 6>: for N <= 48 (the 40-class logits): the B tiles shrink to 6 KB, two more stages fit (the narrow
 //                   GEMM is bound by the DRAM latency of A, so depth is what it needs) and the MMAs do 3/8 of the work.
+//   BatchNorm-backward with TMA-staged Xout / Y <128, 2, XY_BYTES>: the 64 KB of Xout / Y leave room for 2 stages.
 template <int BN_T, int NSTAGE, int EXTRA = 0>
 struct Cfg {
   static constexpr int BN = BN_T, STAGES = NSTAGE;
   static constexpr int B_TILE_BYTES = BN_T * BK * 4;
-  static constexpr int STAGE_BYTES = 2 * TILE_BYTES + 2 * B_TILE_BYTES;          // A_hi, A_lo, B_hi, B_lo
+  static constexpr int STAGE_BYTES = TILE_BYTES + 2 * B_TILE_BYTES;              // A, B_hi, B_lo
   static constexpr int ACC = BN_T / 2;                                            // accumulator registers per thread
   static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + BAR_BYTES + EPI_BYTES + STAT_BYTES + EXTRA + 1024;  // + alignment slack
   static_assert(B_TILE_BYTES % 1024 == 0 && (BN_T == 128 || BN_T == 48), "tile shape (wgmma wrappers: N = 128, 48)");
@@ -60,8 +63,21 @@ struct Cfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory");
 };
 
-__device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t s) { wgmma_tf32_n128(d, a, b, s); }
-__device__ __forceinline__ void mma(float (&d)[24], uint64_t a, uint64_t b, uint32_t s) { wgmma_tf32_n48(d, a, b, s); }
+__device__ __forceinline__ void mma(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_tf32_n128_rs(d, a, b, s); }
+__device__ __forceinline__ void mma(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_tf32_n48_rs(d, a, b, s); }
+
+// This thread's wgmma A fragments of one stage: v[k][i] = row r0 + 8 (i % 2), column 8 k + lane % 4 + 4 (i / 2) of the
+// 128B-swizzled [128][32] A tile, r0 = 16 (consumer warp) + lane / 4.  The rows of one load differ in r0 % 8 = lane / 4,
+// so the swizzle puts the 8 row groups in 8 different 16-byte chunks: 32 banks.  `frag` = a_frag_offset(...) + the
+// tile's shared address (1024-byte aligned), so the swizzled chunk is one XOR away.
+__device__ __forceinline__ uint32_t a_frag_offset(int r0, int lane) { return r0 * 128 + ((lane >> 2) << 4) + (lane & 3) * 4; }
+__device__ __forceinline__ void load_a(uint32_t frag, uint32_t (&v)[BK / 8][4]) {
+  asm("" : "+r"(frag));   // opaque: one XOR per load instead of 8 swizzled offsets held in registers across the epilogue
+#pragma unroll
+  for (int k = 0; k < BK / 8; ++k)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[k][i] = lds32((frag ^ ((2 * k + (i >> 1)) << 4)) + (i & 1) * 8 * 128);
+}
 
 // float index of 16-byte chunk c4 (0..7) of row r in a warp's [16][32] staging block
 __device__ __forceinline__ int stg(int r, int c4) { return r * 32 + ((c4 ^ (r & 7)) << 2); }
@@ -157,8 +173,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           uint8_t* st = smem + s * STAGE_BYTES;
           mbar_expect_tx(&full[s], TILE_BYTES + 2 * B_TILE_BYTES);
           tma_load_2d(&tmA, &full[s], st, kb * BK, m0);
-          tma_load_2d(&tmBhi, &full[s], st + 2 * TILE_BYTES, kb * BK, n0);
-          tma_load_2d(&tmBlo, &full[s], st + 2 * TILE_BYTES + B_TILE_BYTES, kb * BK, n0);
+          tma_load_2d(&tmBhi, &full[s], st + TILE_BYTES, kb * BK, n0);
+          tma_load_2d(&tmBlo, &full[s], st + TILE_BYTES + B_TILE_BYTES, kb * BK, n0);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
@@ -168,8 +184,6 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   regs_inc<232>();
 
   // -------------------------------------------------------------------- consumers
-  const int cw = (warp >> 2) - 1;                 // warpgroup: rows [64 cw, 64 cw + 64) of the tile
-  const int t = threadIdx.x & 127;
   const int q = warp - 4;                         // consumer warp: rows [16 q, 16 q + 16)
   const bool vec_ok = PEER ? true : ((p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0));
   float* stat = stat_smem + q * (2 * STAT_MAX_N);  // this warp's [2][N] column accumulators
@@ -198,31 +212,26 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
   }
   float acc[ACC], sum[ACC];
+  // A fragments (hi, lo) of two consecutive stages: stage kb's are written while the wgmmas of stage kb - 1, which read
+  // the other set, are in flight
+  uint32_t ah0[BK / 8][4], al0[BK / 8][4], ah1[BK / 8][4], al1[BK / 8][4];
+  const uint32_t frag = a_frag_offset(q * 16 + (lane >> 2), lane);
   int s = 0; uint32_t ph = 0;
   int g_chunk = 0;                                 // running chunk index of this warp (XYTMA slot = g & 1, phase = (g >> 1) & 1)
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
 #pragma unroll
-    for (int i = 0; i < ACC; ++i) sum[i] = 0.f;
+    for (int i = 0; i < ACC; ++i) sum[i] = acc[i] = 0.f;   // acc: not live across the previous tile's epilogue
     int prev = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
+    auto stage = [&](int kb, uint32_t (&h)[BK / 8][4], uint32_t (&l)[BK / 8][4]) {
       mbar_wait(&full[s], ph);
       uint8_t* st = smem + s * STAGE_BYTES;
-      {                                            // split this warpgroup's 64 rows: A -> (A_hi in place, A_lo)
-        uint4* hi = reinterpret_cast<uint4*>(st + cw * WG_TILE_BYTES);
-        uint4* lo = reinterpret_cast<uint4*>(st + TILE_BYTES + cw * WG_TILE_BYTES);
+      load_a(smem_u32(st) + frag, h);
 #pragma unroll
-        for (int i = 0; i < WG_TILE_BYTES / 16 / 128; ++i) {
-          const int o = i * 128 + t;
-          const uint4 v = hi[o];
-          uint4 h, l;
-          split4(v, h, l);
-          hi[o] = h;
-          lo[o] = l;
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> tensor-core reads
-      named_sync(1 + cw, 128);
+      for (int k = 0; k < BK / 8; ++k)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) split1(h[k][i], h[k][i], l[k][i]);
+      reg_fence(h); reg_fence(l);                  // split before the wait: it overlaps the previous stage's wgmmas
       if (kb > 0) {                                // the previous stage's wgmmas have retired: promote, free its stage
         wgmma_wait<0>();
         acc_fence(acc);
@@ -231,27 +240,24 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         mbar_arrive(&empty[prev]);
       }
       wgmma_fence();
-      const uint32_t sa = smem_u32(st);
+      const uint32_t sb = smem_u32(st + TILE_BYTES);
       // all 8 small correction terms of the stage first, then the 4 large ones: the accumulator is large (and its
       // truncating accumulate costs the most) for 4 of the 12 updates only
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k) {
         const uint32_t koff = k * 32;              // 32 B per K-step inside the 128 B swizzle row
-        const uint64_t a_hi = make_desc_k128(sa + cw * WG_TILE_BYTES + koff);
-        const uint64_t a_lo = make_desc_k128(sa + TILE_BYTES + cw * WG_TILE_BYTES + koff);
-        const uint64_t b_hi = make_desc_k128(sa + 2 * TILE_BYTES + koff);
-        const uint64_t b_lo = make_desc_k128(sa + 2 * TILE_BYTES + B_TILE_BYTES + koff);
-        mma(acc, a_lo, b_hi, k != 0);
-        mma(acc, a_hi, b_lo, 1);
+        mma(acc, l[k], make_desc_k128(sb + koff), k != 0);
+        mma(acc, h[k], make_desc_k128(sb + B_TILE_BYTES + koff), 1);
       }
 #pragma unroll
-      for (int k = 0; k < BK / 8; ++k) {
-        const uint32_t koff = k * 32;
-        mma(acc, make_desc_k128(sa + cw * WG_TILE_BYTES + koff), make_desc_k128(sa + 2 * TILE_BYTES + koff), 1);
-      }
+      for (int k = 0; k < BK / 8; ++k) mma(acc, h[k], make_desc_k128(sb + k * 32), 1);
       wgmma_commit();
       prev = s;
       if (++s == STAGES) { s = 0; ph ^= 1; }
+    };
+    for (int kb = 0; kb < num_kb; kb += 2) {
+      stage(kb, ah0, al0);
+      if (kb + 1 < num_kb) stage(kb + 1, ah1, al1);
     }
     wgmma_wait<0>();
     acc_fence(acc);
@@ -462,14 +468,14 @@ static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const f
     if (N % 32 || N > gemm::STAT_MAX_N || N <= 48 || ldc % 4 || !aligned_to(C, 16) || !st->stat_partial) return B200GNN_ERR_UNSUPPORTED;
     p.stat_mode = st->stat_mode; p.stat_partial = st->stat_partial; p.bn_x = st->bn_x; p.bn_y = st->bn_y;
     p.bn_mean = st->bn_mean; p.bn_invstd = st->bn_invstd; p.inv_keep = st->inv_keep;
-    if (p.stat_mode == 1) return gemm::launch<gemm::Cfg<128, 3>, 1>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    if (p.stat_mode == 1) return gemm::launch<gemm::Cfg<128, 4>, 1>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
     // BatchNorm-backward epilogue: Xout / Y staged through TMA (two chunks in flight per warp) when every chunk is whole
     if (N % 128 == 0 && (g_bnbwd_variant == 1 || (g_bnbwd_variant == 0 && K < gemm::BNBWD_TMA_MAX_K)))
       return gemm::launch<gemm::Cfg<128, 2, gemm::XY_BYTES>, 3>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
-    return gemm::launch<gemm::Cfg<128, 3>, 2>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    return gemm::launch<gemm::Cfg<128, 4>, 2>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
   }
-  if (N <= 48) return gemm::launch<gemm::Cfg<48, 4>>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
-  return gemm::launch<gemm::Cfg<128, 3>>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  return gemm::launch<gemm::Cfg<128, 4>>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
 }
 
 // Slots of the statistics partial buffer the fused GEMMs below fill: [slots][2][N] floats.
@@ -540,7 +546,7 @@ extern "C" int b200gnn_gemm_tf32x3_scatter_f32(const float* A, int64_t lda, cons
     if (!C_ptrs[q] || !aligned_to(C_ptrs[q], 16)) return B200GNN_ERR_BAD_ARG;
     p.Cp[q] = C_ptrs[q];
   }
-  return gemm::launch<gemm::Cfg<128, 3>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  return gemm::launch<gemm::Cfg<128, 4>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
 }
 
 // C = A · B^T (+bias) stored to EVERY destination buffer C_ptrs[q] (row pitch ldc floats) at rows row_off + m: the row
@@ -559,6 +565,6 @@ extern "C" int b200gnn_gemm_tf32x3_bcast_f32(const float* A, int64_t lda, const 
     if (!C_ptrs[q] || !aligned_to(C_ptrs[q], 16)) return B200GNN_ERR_BAD_ARG;
     p.Cp[q] = C_ptrs[q];
   }
-  if (N <= 48) return gemm::launch<gemm::Cfg<48, 4>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
-  return gemm::launch<gemm::Cfg<128, 3>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  return gemm::launch<gemm::Cfg<128, 4>, 0, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
 }

@@ -6,12 +6,14 @@
 // streams its slices of X and G through shared memory exactly once, keeps the tile's partial in registers, and a small
 // second kernel adds the per-range partials in a fixed order (deterministic, no atomics).
 //
-// Both operands are "MN-major" (the contraction index is the slow one in memory), and wgmma takes tf32 operands
-// K-major only.  So the consumers transpose as they split: TMA lands [32 nodes][128 columns] of X and of G, and the
-// 256 consumer threads write (hi, lo) of each as [128 rows][32 nodes] K-major tiles with the 128-byte swizzle, the
-// layout of gemm_tf32x3.cu.  The transposed tiles are double-buffered, so the split of node block i overlaps the
-// wgmmas of block i-1.  Accumulation as in gemm_tf32x3.cu: each block's 12 wgmmas go to a fresh register accumulator
-// that is added (fp32, round to nearest) into the running partial.
+// Both operands are "MN-major" (the contraction index is the slow one in memory).  X^T is the wgmma A operand, which
+// comes from registers: TMA lands X as 16 boxes of [32 nodes][8 columns], and every consumer thread loads its fragment
+// straight from them (conflict-free: the 4 nodes of one load are 32 bytes apart) and splits it in registers.  G is the
+// B operand, which wgmma reads from shared memory K-major only, so the consumers transpose it as they split: TMA lands
+// [32 nodes][128 columns] of G and the 256 consumer threads write (hi, lo) as [128 rows][32 nodes] K-major tiles with
+// the 128-byte swizzle, the layout of gemm_tf32x3.cu.  The transposed tiles and the X fragments are double-buffered,
+// so the split of node block i overlaps the wgmmas of block i-1.  Accumulation as in gemm_tf32x3.cu: each block's 12
+// wgmmas go to a fresh register accumulator that is added (fp32, round to nearest) into the running partial.
 //
 // 384 threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the tile each.
 #include "common.cuh"
@@ -24,10 +26,11 @@ using namespace tc;
 constexpr int BKN = 32;                       // nodes per stage: one 128-byte K-major row of the transposed operands
 constexpr int TM = 128, TN = 128;             // output tile (rows of dW = columns of X, columns of dW = columns of G)
 constexpr int THREADS = 384;
-constexpr int STAGES = 3;
-constexpr int RAW_BYTES = BKN * (TM + TN) * 4;   // 32 KB: X and G blocks as TMA lands them, [node][column]
+constexpr int STAGES = 5;
+constexpr int X_BOX = 8;                         // X lands as TM / X_BOX boxes of [BKN nodes][X_BOX columns]
+constexpr int RAW_BYTES = BKN * (TM + TN) * 4;   // 32 KB: X and G blocks as TMA lands them
 constexpr int OP_BYTES = 128 * BKN * 4;          // 16 KB: one transposed operand, [128 rows][32 nodes]
-constexpr int T_BYTES = 4 * OP_BYTES;            // X_hi, X_lo, G_hi, G_lo
+constexpr int T_BYTES = 2 * OP_BYTES;            // G_hi, G_lo
 constexpr int SMEM_BYTES = STAGES * RAW_BYTES + 2 * T_BYTES + 256 + 1024;
 constexpr int MAX_RANGES = 132;                  // node ranges (workspace partials): one CTA per SM over all tiles
 // The workspace holds at most the partials of the largest shape of the 128/256-wide layers (132 ranges of 256 x 256);
@@ -71,7 +74,8 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
         mbar_wait(&empty[s], ph ^ 1);
         uint8_t* st = smem + s * RAW_BYTES;
         mbar_expect_tx(&full[s], RAW_BYTES);
-        tma_load_2d(&tmX, &full[s], st, mt * TM, kb * BKN);
+        for (int j = 0; j < TM / X_BOX; ++j)
+          tma_load_2d(&tmX, &full[s], st + j * BKN * X_BOX * 4, mt * TM + j * X_BOX, kb * BKN);
         tma_load_2d(&tmG, &full[s], st + BKN * TM * 4, nt * TN, kb * BKN);
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
@@ -82,30 +86,38 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
 
   const int cw = (warp >> 2) - 1;             // warpgroup: rows [64 cw, 64 cw + 64) of the tile
   const int ct = threadIdx.x - 128;           // 0..255
+  // X^T fragment of this thread: register i of k-step k is row (column of X) 64 cw + 16 (warp % 4) + lane / 4 + 8 (i % 2),
+  // node 8 k + lane % 4 + 4 (i / 2), i.e. box 8 cw + 2 (warp % 4) + i % 2, column lane / 4 of the box
+  const uint32_t xfrag = (8 * cw + 2 * (warp & 3)) * (BKN * X_BOX * 4) + (lane & 3) * (X_BOX * 4) + (lane >> 2) * 4;
   float acc[64], sum[64];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+  for (int i = 0; i < 64; ++i) sum[i] = acc[i] = 0.f;
+  uint32_t xh0[BKN / 8][4], xl0[BKN / 8][4], xh1[BKN / 8][4], xl1[BKN / 8][4];   // X fragments of two consecutive blocks
   int s = 0; uint32_t ph = 0;
-  for (int kb = kb0, i = 0; kb < kb1; ++kb, ++i) {
+  auto block = [&](int i, uint32_t (&h)[BKN / 8][4], uint32_t (&l)[BKN / 8][4]) {
     mbar_wait(&full[s], ph);
-    const float* rx = reinterpret_cast<const float*>(smem + s * RAW_BYTES);   // [32 nodes][128]
-    const float* rg = rx + BKN * TM;
+    const uint32_t sraw = smem_u32(smem + s * RAW_BYTES);
+    const float* rg = reinterpret_cast<const float*>(smem + s * RAW_BYTES + BKN * TM * 4);   // [32 nodes][128]
     uint8_t* T = tbuf + (i & 1) * T_BYTES;
-    // transpose + split: item = (operand, row r, 4-node chunk c); consecutive threads take consecutive rows, so the
+    // transpose + split of G: item = (row r, 4-node chunk c); consecutive threads take consecutive rows, so the
     // reads are conflict-free and the 16-byte swizzled writes of 8 consecutive rows cover all banks
 #pragma unroll
-    for (int u = 0; u < 8; ++u) {
+    for (int u = 0; u < 4; ++u) {
       const int idx = u * 256 + ct;
-      const int op = idx >> 10, r = idx & 127, c = (idx >> 7) & 7;
-      const float* src = (op ? rg : rx) + (4 * c) * 128 + r;
+      const int r = idx & 127, c = idx >> 7;
+      const float* src = rg + (4 * c) * 128 + r;
       const uint4 v = make_uint4(__float_as_uint(src[0]), __float_as_uint(src[128]), __float_as_uint(src[256]),
                                  __float_as_uint(src[384]));
-      uint4 h, l;
-      split4(v, h, l);
-      uint8_t* base = T + op * 2 * OP_BYTES;
-      *reinterpret_cast<uint4*>(base + swz128(r, c)) = h;
-      *reinterpret_cast<uint4*>(base + OP_BYTES + swz128(r, c)) = l;
+      uint4 hv, lv;
+      split4(v, hv, lv);
+      *reinterpret_cast<uint4*>(T + swz128(r, c)) = hv;
+      *reinterpret_cast<uint4*>(T + OP_BYTES + swz128(r, c)) = lv;
     }
+#pragma unroll
+    for (int k = 0; k < BKN / 8; ++k)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        split1(lds32(sraw + xfrag + (j & 1) * (BKN * X_BOX * 4) + (8 * k + 4 * (j >> 1)) * (X_BOX * 4)), h[k][j], l[k][j]);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     mbar_arrive(&empty[s]);                    // the raw block has been read
     if (i > 0) {                               // block i-1's wgmmas have retired: promote
@@ -115,25 +127,23 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
       for (int j = 0; j < 64; ++j) sum[j] += acc[j];
     }
     named_sync(1, 256);                        // T[i & 1] complete; every warpgroup is done with T[(i + 1) & 1]
+    reg_fence(h); reg_fence(l);
     wgmma_fence();
     const uint32_t sa = smem_u32(T);
 #pragma unroll
     for (int k = 0; k < BKN / 8; ++k) {        // the small correction terms first (see gemm_tf32x3.cu)
       const uint32_t koff = k * 32;
-      const uint64_t x_hi = make_desc_k128(sa + cw * (OP_BYTES / 2) + koff);
-      const uint64_t x_lo = make_desc_k128(sa + OP_BYTES + cw * (OP_BYTES / 2) + koff);
-      const uint64_t g_hi = make_desc_k128(sa + 2 * OP_BYTES + koff);
-      const uint64_t g_lo = make_desc_k128(sa + 3 * OP_BYTES + koff);
-      wgmma_tf32_n128(acc, x_lo, g_hi, k != 0);
-      wgmma_tf32_n128(acc, x_hi, g_lo, 1);
+      wgmma_tf32_n128_rs(acc, l[k], make_desc_k128(sa + koff), k != 0);
+      wgmma_tf32_n128_rs(acc, h[k], make_desc_k128(sa + OP_BYTES + koff), 1);
     }
 #pragma unroll
-    for (int k = 0; k < BKN / 8; ++k) {
-      const uint32_t koff = k * 32;
-      wgmma_tf32_n128(acc, make_desc_k128(sa + cw * (OP_BYTES / 2) + koff), make_desc_k128(sa + 2 * OP_BYTES + koff), 1);
-    }
+    for (int k = 0; k < BKN / 8; ++k) wgmma_tf32_n128_rs(acc, h[k], make_desc_k128(sa + k * 32), 1);
     wgmma_commit();
     if (++s == STAGES) { s = 0; ph ^= 1; }
+  };
+  for (int i = 0; i < kb1 - kb0; i += 2) {
+    block(i, xh0, xl0);
+    if (i + 1 < kb1 - kb0) block(i + 1, xh1, xl1);
   }
   if (kb1 > kb0) {
     wgmma_wait<0>();
@@ -184,13 +194,13 @@ __global__ void __launch_bounds__(RED_VECS * RED_GROUPS) wgrad_reduce_kernel(con
   *reinterpret_cast<float4*>(out + (size_t)row * Nout + c4) = acc;   // Nout % 4 == 0
 }
 
-// [rows, width] fp32 row-major (ld): boxes of 128 columns x BKN rows, no swizzle, zero fill past the last row / column
-static bool make_map_rows(CUtensorMap* m, const float* base, int64_t rows, int64_t width, int64_t ld) {
+// [rows, width] fp32 row-major (ld): boxes of box_cols columns x BKN rows, no swizzle, zero fill past the last row / column
+static bool make_map_rows(CUtensorMap* m, const float* base, int64_t rows, int64_t width, int64_t ld, int box_cols) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return false;
   cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {128, (cuuint32_t)BKN};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)BKN};
   cuuint32_t estr[2] = {1, 1};
   return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -226,7 +236,8 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const 
       !aligned_to(dW, 16) || !aligned_to(workspace, 16))
     return B200GNN_ERR_UNSUPPORTED;
   CUtensorMap tX, tG;
-  if (!wgrad::make_map_rows(&tX, X, Nn, Kin, ldx) || !wgrad::make_map_rows(&tG, G, Nn, Nout, ldg)) return B200GNN_ERR_UNSUPPORTED;
+  if (!wgrad::make_map_rows(&tX, X, Nn, Kin, ldx, wgrad::X_BOX) || !wgrad::make_map_rows(&tG, G, Nn, Nout, ldg, wgrad::TN))
+    return B200GNN_ERR_UNSUPPORTED;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device
