@@ -818,12 +818,14 @@ __global__ void __launch_bounds__(256) spmm_hub_finalize_kernel(const SpmmParams
     }
     return;
   }
+  // scalar path (K % 4 != 0, K > 1024 or a misaligned operand); in scatter mode the row goes to its rank's buffer
+  float* yrow = p.n_yp ? reinterpret_cast<float*>(y_row_v4(p, row)) : p.Y + (size_t)row * p.ldy;
   for (int k = threadIdx.x; k < p.K; k += blockDim.x) {
     float acc = 0.f;
     for (int s = s0; s < s1; ++s) acc += p.hub_ws[(size_t)s * p.K + k];
     if (p.mean) acc /= (float)max(deg, 1);
     if (p.bias) acc += __ldg(p.bias + k);
-    p.Y[(size_t)row * p.ldy + k] = acc;
+    yrow[k] = acc;
     if (stat) { stat[k] = acc; stat[p.K + k] = acc * acc; }
   }
 }
@@ -1110,8 +1112,11 @@ extern "C" int b200gnn_spmm_csr_f32(const int32_t* rowptr, const int32_t* col, c
   p.n_yp = 0; p.ycol = 0; p.ldyp = 0;
   if (g_scatter.n > 0) {            // set by b200gnn_spmm_csr_scatter_f32 around this call (same thread)
     if (W != 4 || K % 4 || g_scatter.ld % 4 || g_scatter.col % 4) return B200GNN_ERR_UNSUPPORTED;
-    const bool ok_kernel = (K % 128 == 0 && K <= 4096) || (p.nvec <= 16 && !stat_partial);
-    if (!ok_kernel || (g_spmm_variant & 15) == 1 || (g_spmm_variant & 15) == 2) return B200GNN_ERR_UNSUPPORTED;
+    // only the bulk-copy kernels (automatic choice or families 3-7) and the narrow kernel store through y_row_v4
+    const int sfam = g_spmm_variant & 15;
+    const bool to_bulk = K % 128 == 0 && K <= 4096 && (sfam == 0 || (sfam >= 3 && sfam <= 7));
+    const bool to_narrow = p.nvec <= 16 && !stat_partial && sfam != 1 && sfam != 2;
+    if (!to_bulk && !to_narrow) return B200GNN_ERR_UNSUPPORTED;
     p.n_yp = g_scatter.n; p.ycol = (int32_t)g_scatter.col; p.ldyp = g_scatter.ld;
     for (int q = 0; q < g_scatter.n; ++q) { p.Yp[q] = g_scatter.ptr[q]; p.yoff[q] = g_scatter.off[q]; }
     p.yoff[g_scatter.n] = g_scatter.off[g_scatter.n];

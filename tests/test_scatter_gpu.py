@@ -37,10 +37,11 @@ def test_gemm_epilogue_r2c_scatter(world, N, K):
         assert torch.isnan(dst[q][:row_off]).all() and torch.isnan(dst[q][row_off + M:]).all()
 
 
-@pytest.mark.parametrize("world,K", [(2, 128), (4, 256), (8, 32), (8, 16), (2, 64)])
+@pytest.mark.parametrize("world,K", [(2, 128), (4, 256), (8, 32), (8, 16), (2, 64), (2, 1152), (4, 2048)])
 def test_spmm_epilogue_c2r_scatter(world, K):
     """b200gnn_spmm_csr_scatter_f32 on the TMA kernels (K % 128 == 0) and the narrow kernel, hub rows included: row i goes to
-    the buffer of the rank owning it at (i - off[q], col_dst ...)."""
+    the buffer of the rank owning it at (i - off[q], col_dst ...).  K = 1152 / 2048 (> 1024) finish the hub rows on the hub
+    finalize's scalar path."""
     n = 20_000
     gen = torch.Generator().manual_seed(5)
     hub = torch.randperm(n, generator=gen)[:5000]
