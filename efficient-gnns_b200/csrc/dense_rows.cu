@@ -268,6 +268,60 @@ __global__ void __launch_bounds__(256) dropout_mask_kernel(uint8_t* __restrict__
   }
 }
 
+// The same keep decisions packed one bit per element for n_layers hidden layers at once: layer l (offset + l, plus
+// step_dev * step_mul) fills bits[l][row][w], bit b = column 32 w + b (zero past K).  One thread per word; consecutive float4s
+// of a word share their Philox block in the P16 path.  The GEMMs recompute the activation from Y and these bits
+// (b200gnn_gemm_tf32x3_act_f32 and friends), so the [n_rows, K] activation is never written.
+__global__ void __launch_bounds__(256) dropout_bits_kernel(uint32_t* __restrict__ bits, int n_layers, int64_t n_rows, int nvec_row,
+                                                           int words, float p, int p16, uint32_t thr16, uint64_t seed,
+                                                           uint64_t offset, const int32_t* __restrict__ step_dev,
+                                                           uint64_t step_mul) {
+  if (step_dev) offset += (uint64_t)(*step_dev) * step_mul;
+  const int64_t per_layer = n_rows * words;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < per_layer * n_layers; t += (int64_t)gridDim.x * blockDim.x) {
+    const int layer = (int)(t / per_layer);
+    const int64_t e = t - layer * per_layer, row = e / words;
+    const int w = (int)(e - row * words);
+    const uint64_t off = offset + (uint64_t)layer;
+    uint32_t out = 0u;
+    uint64_t blk = ~0ull;
+    uint4 r = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int cv = 8 * w + j;
+      if (cv >= nvec_row) break;
+      const uint64_t g = (uint64_t)row * nvec_row + cv;
+      uchar4 m;
+      if (p16) {
+        if ((g >> 1) != blk) { blk = g >> 1; r = philox4x32(seed, off, blk); }
+        m = keep16((g & 1) ? r.z : r.x, (g & 1) ? r.w : r.y, thr16);
+      } else {
+        m = keep24(philox4x32(seed, off, g), p);
+      }
+      out |= ((uint32_t)m.x | ((uint32_t)m.y << 1) | ((uint32_t)m.z << 2) | ((uint32_t)m.w << 3)) << (4 * j);
+    }
+    bits[t] = out;
+  }
+}
+
+// out = bit ? relu(y*scale + shift) / (1-p) : 0 — the activation the fused GEMMs use, materialised (same operations as
+// affine_relu_dropout_kernel, so bit-identical to it for the same keep decisions).
+__global__ void __launch_bounds__(256) affine_relu_bits_kernel(const float* __restrict__ Y, const uint32_t* __restrict__ bits,
+                                                               const float* __restrict__ scale, const float* __restrict__ shift,
+                                                               float* __restrict__ out, int64_t n_vec, int nvec_row, int words,
+                                                               float p) {
+  const float inv_keep = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t row = i / nvec_row;
+    const int cv = (int)(i - row * nvec_row);
+    float4 y = affine_relu4(ld4(Y + 4 * i), scale, shift, cv, 1);
+    const uint32_t b = bits[row * words + (cv >> 3)] >> (4 * (cv & 7));
+    y.x = (b & 1u) ? y.x * inv_keep : 0.f; y.y = (b & 2u) ? y.y * inv_keep : 0.f;
+    y.z = (b & 4u) ? y.z * inv_keep : 0.f; y.w = (b & 8u) ? y.w * inv_keep : 0.f;
+    st4(out + 4 * i, y);
+  }
+}
+
 // p * 65536 integral (and p > 0): the 16-bit decision path is exact
 static inline bool dropout_p16(float p, uint32_t& thr16) {
   const double t = (double)p * 65536.0;
@@ -534,6 +588,30 @@ extern "C" int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K,
   uint32_t thr16 = 0;
   const int p16 = dropout_p16(p, thr16) ? 1 : 0;
   dropout_mask_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(mask, n_vec, p, p16, thr16, seed, offset);
+  return check_launch();
+}
+
+extern "C" int b200gnn_dropout_bits_u32(uint32_t* bits, int64_t n_layers, int64_t n_rows, int64_t K, float p, uint64_t seed,
+                                        uint64_t offset, const int32_t* step_dev, uint64_t step_mul, void* stream) {
+  if (!rows_ok(n_rows, K) || !bits || n_layers < 1 || p < 0.f || p >= 1.f) return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  const int words = (int)((K + 31) / 32);
+  uint32_t thr16 = 0;
+  const int p16 = dropout_p16(p, thr16) ? 1 : 0;
+  dropout_bits_kernel<<<grid_for(n_layers * n_rows * words, 256 * 2), 256, 0, (cudaStream_t)stream>>>(
+      bits, (int)n_layers, n_rows, (int)(K / 4), words, p, p16, thr16, seed, offset, step_dev, step_mul);
+  return check_launch();
+}
+
+extern "C" int b200gnn_affine_relu_bits_f32(const float* Y, const uint32_t* bits, const float* scale, const float* shift,
+                                            float p, float* out, int64_t n_rows, int64_t K, void* stream) {
+  if (!rows_ok(n_rows, K) || !Y || !bits || !scale || !shift || !out || p < 0.f || p >= 1.f || !aligned_to(Y, 16) ||
+      !aligned_to(out, 16) || !aligned_to(scale, 16) || !aligned_to(shift, 16))
+    return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  const int64_t n_vec = n_rows * (K / 4);
+  affine_relu_bits_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(Y, bits, scale, shift, out, n_vec,
+                                                                                     (int)(K / 4), (int)((K + 31) / 32), p);
   return check_launch();
 }
 

@@ -109,10 +109,22 @@ struct Params {
   const float* bn_mean;
   const float* bn_invstd;
   float inv_keep;
+  // ACT: the activation A = dropout(relu(Y * scale + shift)) of a hidden layer is recomputed from Y, the per-column
+  // scale / shift of its BatchNorm and the packed keep bits (uint32 [rows][act_words], bit c % 32 of word c / 32 is the
+  // dropout decision of column c) instead of being read:
+  //   stat_mode 0: the A operand is Y, and every A fragment element becomes bit ? max(y * scale + shift, 0) * inv_keep : 0
+  //                before its tf32 split (the same operations as b200gnn_affine_relu_dropout_f32, so the product is that of
+  //                the materialised activation bit for bit);
+  //   stat_mode 2: the mask [Xout > 0] of the BatchNorm-backward epilogue becomes bit && y * scale + shift > 0 (bn_x unused).
+  const float* act_scale;
+  const float* act_shift;
+  const uint32_t* act_bits;
+  int32_t act_words;
 };
 
 // stat_mode 2: the pieces of Xout / Y one lane needs for a 32-column chunk (4 rows x 4 columns: rows it*4 + lane/8
 // of the warp's 16 rows, columns 4*(lane%8)...) — the same row segments its stores cover.
+template <bool ACT>
 __device__ __forceinline__ void load_bn_chunk(const Params& p, int m0, int col, int q, int lane, float4 (&x)[4], float4 (&y)[4]) {
   if (col + 32 > p.N) return;
   const int sub = lane >> 3, cq = (lane & 7) * 4;
@@ -121,15 +133,31 @@ __device__ __forceinline__ void load_bn_chunk(const Params& p, int m0, int col, 
     const int grow = m0 + q * 16 + it * 4 + sub;
     if (grow < p.M) {
       const size_t o = (size_t)grow * p.ldc + col + cq;
-      x[it] = __ldg(reinterpret_cast<const float4*>(p.bn_x + o));
+      if (!ACT) x[it] = __ldg(reinterpret_cast<const float4*>(p.bn_x + o));
       y[it] = __ldg(reinterpret_cast<const float4*>(p.bn_y + o));
     }
   }
 }
 
-// STAT: 0 plain, 1 / 2 the fused column reductions (Params::stat_mode); PEER: the output goes to peer buffers (Params::Cp).
-// Compile-time so that each instantiation carries only its own epilogue (the epilogue is the hot loop of the narrow-K GEMMs).
-template <class C, int STAT, bool PEER>
+// ACT with stat_mode 2: this lane's keep words of a 32-column chunk (one word: chunks are 32-column aligned), rows as above
+__device__ __forceinline__ void load_bits_chunk(const Params& p, int m0, int col, int q, int lane, uint32_t (&w)[4]) {
+  const int sub = lane >> 3;
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int grow = m0 + q * 16 + it * 4 + sub;
+    w[it] = grow < p.M ? __ldg(p.act_bits + (size_t)grow * p.act_words + (col >> 5)) : 0u;
+  }
+}
+
+// ACT with stat_mode 0: the activation of one A element from y, its column's (scale, shift) and its keep bit
+__device__ __forceinline__ uint32_t act1(uint32_t y, float sc, float sh, uint32_t keep, float inv_keep) {
+  return keep ? __float_as_uint(fmaxf(fmaf(__uint_as_float(y), sc, sh), 0.f) * inv_keep) : 0u;
+}
+
+// STAT: 0 plain, 1 / 2 the fused column reductions (Params::stat_mode); PEER: the output goes to peer buffers (Params::Cp);
+// ACT: the hidden activation is recomputed from Y (Params::act_bits).  Compile-time so that each instantiation carries only
+// its own prologue and epilogue (the epilogue is the hot loop of the narrow-K GEMMs).
+template <class C, int STAT, bool PEER, bool ACT = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                    const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmX,
@@ -205,12 +233,33 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     if (lane == 0)
       for (int g = 0; g < 2 && g < n_mine; ++g) {
         const int tt = blockIdx.x + (g / NCHUNK) * gridDim.x, cc = g % NCHUNK;
-        mbar_expect_tx(&xyb[g], XY_SLOT_BYTES);
-        tma_load_2d(&tmX, &xyb[g], xy + g * XY_SLOT_BYTES, (tt % num_n) * BN + cc * 32, (tt / num_n) * BM + q * XY_ROWS);
+        mbar_expect_tx(&xyb[g], ACT ? XY_SLOT_BYTES / 2 : XY_SLOT_BYTES);
+        if (!ACT)
+          tma_load_2d(&tmX, &xyb[g], xy + g * XY_SLOT_BYTES, (tt % num_n) * BN + cc * 32, (tt / num_n) * BM + q * XY_ROWS);
         tma_load_2d(&tmY, &xyb[g], xy + g * XY_SLOT_BYTES + XY_SLOT_BYTES / 2, (tt % num_n) * BN + cc * 32,
                     (tt / num_n) * BM + q * XY_ROWS);
       }
   }
+  // ACT prologue: the (scale, shift) pairs of all K columns sit in the (otherwise unused) statistics block, ordered so that a
+  // thread's 8 columns of a stage, 8 k + lane % 4 + 4 j, are 4 consecutive float4 {sc(k,0), sh(k,0), sc(k,1), sh(k,1)}
+  const float* act_ss = stat_smem;
+  if (ACT && !STAT) {
+    for (int c = threadIdx.x - 128; c < num_kb * BK; c += 256) {
+      const int w = c & 31;
+      const float2 v = c < p.K ? make_float2(__ldg(p.act_scale + c), __ldg(p.act_shift + c)) : make_float2(0.f, 0.f);
+      *reinterpret_cast<float2*>(stat_smem + (c >> 5) * 64 + (w & 3) * 16 + (w >> 3) * 4 + ((w >> 2) & 1) * 2) = v;
+    }
+    named_sync(1, 256);
+  }
+  // keep words of this thread's two A rows (r0, r0 + 8) for the next stage: fetched one stage ahead
+  const int arow = q * 16 + (lane >> 2);
+  auto act_words = [&](int tile, int kb, uint32_t (&w)[2]) {
+    const int r = (tile / num_n) * BM + arow;
+    w[0] = r < p.M ? __ldg(p.act_bits + (size_t)r * p.act_words + kb) : 0u;
+    w[1] = r + 8 < p.M ? __ldg(p.act_bits + (size_t)(r + 8) * p.act_words + kb) : 0u;
+  };
+  uint32_t wnext[2] = {0u, 0u};
+  if (ACT && !STAT && blockIdx.x < num_tiles) act_words(blockIdx.x, 0, wnext);
   float acc[ACC], sum[ACC];
   // A fragments (hi, lo) of two consecutive stages: stage kb's are written while the wgmmas of stage kb - 1, which read
   // the other set, are in flight
@@ -224,9 +273,26 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     for (int i = 0; i < ACC; ++i) sum[i] = acc[i] = 0.f;   // acc: not live across the previous tile's epilogue
     int prev = 0;
     auto stage = [&](int kb, uint32_t (&h)[BK / 8][4], uint32_t (&l)[BK / 8][4]) {
+      uint32_t wcur[2];
+      if (ACT && !STAT) {
+        wcur[0] = wnext[0] >> (lane & 3); wcur[1] = wnext[1] >> (lane & 3);
+        if (kb + 1 < num_kb) act_words(tile, kb + 1, wnext);
+        else if (tile + (int)gridDim.x < num_tiles) act_words(tile + gridDim.x, 0, wnext);
+      }
       mbar_wait(&full[s], ph);
       uint8_t* st = smem + s * STAGE_BYTES;
       load_a(smem_u32(st) + frag, h);
+      if (ACT && !STAT) {
+        const float4* ss = reinterpret_cast<const float4*>(act_ss + kb * 64 + (lane & 3) * 16);
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k) {
+          const float4 t = ss[k];
+#pragma unroll
+          for (int i = 0; i < 4; ++i)   // element i: row r0 + 8 (i % 2), column 8 k + lane % 4 + 4 (i / 2)
+            h[k][i] = act1(h[k][i], (i >> 1) ? t.z : t.x, (i >> 1) ? t.w : t.y, (wcur[i & 1] >> (8 * k + 4 * (i >> 1))) & 1u,
+                           p.inv_keep);
+        }
+      }
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k)
 #pragma unroll
@@ -271,7 +337,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     for (int c = 0; c < NCHUNK; ++c, ++g_chunk) {
       const int col0 = n0 + c * 32;
       float4 xr[4], yr[4];
-      if (STAT == 2) load_bn_chunk(p, m0, col0, q, lane, xr, yr);
+      if (STAT == 2) load_bn_chunk<ACT>(p, m0, col0, q, lane, xr, yr);
       // accumulator fragment -> staging block, so that global stores are whole 128-byte row segments
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
@@ -291,10 +357,16 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (p.bias) b4 = make_float4(__ldg(p.bias + col0 + cq), __ldg(p.bias + col0 + cq + 1), __ldg(p.bias + col0 + cq + 2),
                                      __ldg(p.bias + col0 + cq + 3));
-        float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f), q4 = s4, mu4 = s4, is4 = s4;
+        float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f), q4 = s4, mu4 = s4, is4 = s4, sc4 = s4, sh4 = s4;
         if (BNB) {
           mu4 = __ldg(reinterpret_cast<const float4*>(p.bn_mean + col0 + cq));
           is4 = __ldg(reinterpret_cast<const float4*>(p.bn_invstd + col0 + cq));
+        }
+        uint32_t wb[4];
+        if (BNB && ACT) {
+          sc4 = __ldg(reinterpret_cast<const float4*>(p.act_scale + col0 + cq));
+          sh4 = __ldg(reinterpret_cast<const float4*>(p.act_shift + col0 + cq));
+          load_bits_chunk(p, m0, col0, q, lane, wb);
         }
 #pragma unroll
         for (int it = 0; it < 4; ++it) {
@@ -317,10 +389,19 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             if (STAT == 1) {
               vstat(s4, q4, v);
             } else if (BNB) {
-              const float4 x = XYTMA ? *reinterpret_cast<const float4*>(xs + rr * 32 + cq) : xr[it];
+              float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (!ACT) x = XYTMA ? *reinterpret_cast<const float4*>(xs + rr * 32 + cq) : xr[it];
               const float4 y = XYTMA ? *reinterpret_cast<const float4*>(ys + rr * 32 + cq) : yr[it];
-              v.x = x.x > 0.f ? v.x * p.inv_keep : 0.f; v.y = x.y > 0.f ? v.y * p.inv_keep : 0.f;
-              v.z = x.z > 0.f ? v.z * p.inv_keep : 0.f; v.w = x.w > 0.f ? v.w * p.inv_keep : 0.f;
+              if (ACT) {                          // Xout > 0  <=>  kept && y * scale + shift > 0
+                const uint32_t b = wb[it] >> cq;
+                v.x = (b & 1u) && fmaf(y.x, sc4.x, sh4.x) > 0.f ? v.x * p.inv_keep : 0.f;
+                v.y = (b & 2u) && fmaf(y.y, sc4.y, sh4.y) > 0.f ? v.y * p.inv_keep : 0.f;
+                v.z = (b & 4u) && fmaf(y.z, sc4.z, sh4.z) > 0.f ? v.z * p.inv_keep : 0.f;
+                v.w = (b & 8u) && fmaf(y.w, sc4.w, sh4.w) > 0.f ? v.w * p.inv_keep : 0.f;
+              } else {
+                v.x = x.x > 0.f ? v.x * p.inv_keep : 0.f; v.y = x.y > 0.f ? v.y * p.inv_keep : 0.f;
+                v.z = x.z > 0.f ? v.z * p.inv_keep : 0.f; v.w = x.w > 0.f ? v.w * p.inv_keep : 0.f;
+              }
               s4.x += v.x; s4.y += v.y; s4.z += v.z; s4.w += v.w;
               q4.x = fmaf(v.x, (y.x - mu4.x) * is4.x, q4.x); q4.y = fmaf(v.y, (y.y - mu4.y) * is4.y, q4.y);
               q4.z = fmaf(v.z, (y.z - mu4.z) * is4.z, q4.z); q4.w = fmaf(v.w, (y.w - mu4.w) * is4.w, q4.w);
@@ -350,8 +431,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         if (XYTMA && lane == 0 && g_chunk + 2 < n_mine) {      // the slot has been read by every lane: refill it
           const int g = g_chunk + 2, tt = blockIdx.x + (g / NCHUNK) * gridDim.x, cc = g % NCHUNK;
           uint8_t* dst = xy + (g & 1) * XY_SLOT_BYTES;
-          mbar_expect_tx(&xyb[g & 1], XY_SLOT_BYTES);
-          tma_load_2d(&tmX, &xyb[g & 1], dst, (tt % num_n) * BN + cc * 32, (tt / num_n) * BM + q * XY_ROWS);
+          mbar_expect_tx(&xyb[g & 1], ACT ? XY_SLOT_BYTES / 2 : XY_SLOT_BYTES);
+          if (!ACT) tma_load_2d(&tmX, &xyb[g & 1], dst, (tt % num_n) * BN + cc * 32, (tt / num_n) * BM + q * XY_ROWS);
           tma_load_2d(&tmY, &xyb[g & 1], dst + XY_SLOT_BYTES / 2, (tt % num_n) * BN + cc * 32, (tt / num_n) * BM + q * XY_ROWS);
         }
       } else {
@@ -408,7 +489,7 @@ static bool make_map(CUtensorMap* m, const float* base, int64_t rows, int64_t co
             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <class C, int STAT = 0, bool PEER = false>
+template <class C, int STAT = 0, bool PEER = false, bool ACT = false>
 static int launch(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb, const Params& p,
                   cudaStream_t stream) {
   CUtensorMap tA, tBh, tBl, tX, tY;
@@ -416,20 +497,21 @@ static int launch(const float* A, int64_t lda, const float* B_hi, const float* B
       !make_map(&tBl, B_lo, p.N, p.K, ldb, C::BN))
     return B200GNN_ERR_UNSUPPORTED;
   tX = tA; tY = tA;                                  // placeholders unless the epilogue stages Xout / Y through TMA
-  if (STAT == 3 && (!make_map(&tX, p.bn_x, p.M, p.N, p.ldc, XY_ROWS, false) || !make_map(&tY, p.bn_y, p.M, p.N, p.ldc, XY_ROWS, false)))
+  if (STAT == 3 && ((!ACT && !make_map(&tX, p.bn_x, p.M, p.N, p.ldc, XY_ROWS, false)) ||
+                    !make_map(&tY, p.bn_y, p.M, p.N, p.ldc, XY_ROWS, false)))
     return B200GNN_ERR_UNSUPPORTED;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device and instantiation; idempotent if two threads race
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
     attr_set[dev] = true;
   }
   const int tiles = ((p.M + BM - 1) / BM) * ((p.N + C::BN - 1) / C::BN);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
-  gemm_tf32x3_kernel<C, STAT, PEER><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
+  gemm_tf32x3_kernel<C, STAT, PEER, ACT><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
   return check_launch();
 }
 
@@ -451,9 +533,11 @@ extern "C" int b200gnn_split_tf32_f32(const float* W, int64_t rows, int64_t cols
 static int g_bnbwd_variant = 0;   // A/B knob: 0 automatic, 1 force the TMA path, 2 force the register path of the BatchNorm-backward epilogue
 extern "C" void b200gnn_gemm_set_bnbwd_variant(int v) { g_bnbwd_variant = v; }
 
+// st: the fused column statistics (stat_mode 1 / 2); act: the activation recomputed from Y (Params::act_*, inv_keep) — of the
+// A operand without st, of the BatchNorm-backward mask with stat_mode 2.
 static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb, float* C, int64_t ldc,
                          int64_t M, int64_t N, int64_t K, const float* bias, int accumulate, void* stream,
-                         const gemm::Params* st = nullptr) {
+                         const gemm::Params* st = nullptr, const gemm::Params* act = nullptr) {
   if (!A || !B_hi || !B_lo || !C || M <= 0 || N <= 0 || K <= 0 || lda < K || ldb < K || ldc < N ||
       M >= INT32_MAX || N >= INT32_MAX || K >= INT32_MAX)
     return B200GNN_ERR_BAD_ARG;
@@ -463,6 +547,18 @@ static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const f
   gemm::Params p{};
   p.C = C; p.bias = bias; p.ldc = ldc; p.M = (int32_t)M; p.N = (int32_t)N; p.K = (int32_t)K; p.accumulate = accumulate ? 1 : 0;
   p.n_peer = 0; p.kc = 0; p.row_off = 0; p.bcast = 0;
+  if (act) {
+    if (!act->act_scale || !act->act_shift || !act->act_bits || !aligned_to(act->act_scale, 16) || !aligned_to(act->act_shift, 16))
+      return B200GNN_ERR_BAD_ARG;
+    p.act_scale = act->act_scale; p.act_shift = act->act_shift; p.act_bits = act->act_bits; p.act_words = act->act_words;
+    p.inv_keep = act->inv_keep;
+  }
+  if (act && !st) {
+    // (scale, shift) of all K columns in the statistics block of shared memory
+    if (K > (int64_t)gemm::STAT_BYTES / 8) return B200GNN_ERR_UNSUPPORTED;
+    if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>, 0, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    return gemm::launch<gemm::Cfg<128, 4>, 0, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  }
   if (st) {
     // fused column statistics: whole 32-column chunks through the vectorised epilogue only
     if (N % 32 || N > gemm::STAT_MAX_N || N <= 48 || ldc % 4 || !aligned_to(C, 16) || !st->stat_partial) return B200GNN_ERR_UNSUPPORTED;
@@ -470,8 +566,11 @@ static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const f
     p.bn_mean = st->bn_mean; p.bn_invstd = st->bn_invstd; p.inv_keep = st->inv_keep;
     if (p.stat_mode == 1) return gemm::launch<gemm::Cfg<128, 4>, 1>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
     // BatchNorm-backward epilogue: Xout / Y staged through TMA (two chunks in flight per warp) when every chunk is whole
-    if (N % 128 == 0 && (g_bnbwd_variant == 1 || (g_bnbwd_variant == 0 && K < gemm::BNBWD_TMA_MAX_K)))
-      return gemm::launch<gemm::Cfg<128, 2, gemm::XY_BYTES>, 3>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    const bool tma = N % 128 == 0 && (g_bnbwd_variant == 1 || (g_bnbwd_variant == 0 && K < gemm::BNBWD_TMA_MAX_K));
+    if (act)
+      return tma ? gemm::launch<gemm::Cfg<128, 2, gemm::XY_BYTES>, 3, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream)
+                 : gemm::launch<gemm::Cfg<128, 4>, 2, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    if (tma) return gemm::launch<gemm::Cfg<128, 2, gemm::XY_BYTES>, 3>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
     return gemm::launch<gemm::Cfg<128, 4>, 2>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
   }
   if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
@@ -514,6 +613,38 @@ extern "C" int b200gnn_gemm_tf32x3_bnbwd_f32(const float* A, int64_t lda, const 
   st.stat_mode = 2; st.stat_partial = partial; st.bn_x = Xout; st.bn_y = Y; st.bn_mean = mean; st.bn_invstd = invstd;
   st.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
   return gemm_dispatch(A, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, nullptr, accumulate, stream, &st);
+}
+
+// The bnbwd GEMM above for a block whose activation is not materialised: the mask [Xout > 0] is taken from the packed keep
+// bits (uint32 [M][N / 32], as written by b200gnn_dropout_bits_u32) and Y: bit && Y * scale + shift > 0.
+extern "C" int b200gnn_gemm_tf32x3_bnbwd_bits_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                                  float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
+                                                  const uint32_t* bits, const float* Y, const float* mean, const float* invstd,
+                                                  const float* scale, const float* shift, float p_drop, float* partial,
+                                                  int64_t slots, void* stream) {
+  if (!partial || !bits || !Y || !mean || !invstd || p_drop < 0.f || p_drop >= 1.f || slots < b200gnn_gemm_stat_slots(M, N))
+    return B200GNN_ERR_BAD_ARG;
+  if (!aligned_to(Y, 16) || !aligned_to(mean, 16) || !aligned_to(invstd, 16)) return B200GNN_ERR_UNSUPPORTED;
+  gemm::Params st{}, act{};
+  st.stat_mode = 2; st.stat_partial = partial; st.bn_y = Y; st.bn_mean = mean; st.bn_invstd = invstd;
+  st.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  act.act_scale = scale; act.act_shift = shift; act.act_bits = bits; act.act_words = (int32_t)((N + 31) / 32);
+  act.inv_keep = st.inv_keep;
+  return gemm_dispatch(A, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, nullptr, accumulate, stream, &st, &act);
+}
+
+// C = act(Y) · B^T (+ bias), act(Y) = dropout(relu(Y * scale + shift)) with the keep decisions read from the packed bits
+// (uint32 [M][ceil(K / 32)], b200gnn_dropout_bits_u32): bit for bit the GEMM of the activation
+// b200gnn_affine_relu_dropout_f32 would materialise, without that [M, K] tensor.  K <= 2048.
+extern "C" int b200gnn_gemm_tf32x3_act_f32(const float* Y, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                           float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                           const float* scale, const float* shift, const uint32_t* bits, float p_drop,
+                                           void* stream) {
+  if (p_drop < 0.f || p_drop >= 1.f) return B200GNN_ERR_BAD_ARG;
+  gemm::Params act{};
+  act.act_scale = scale; act.act_shift = shift; act.act_bits = bits; act.act_words = (int32_t)((K + 31) / 32);
+  act.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  return gemm_dispatch(Y, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, bias, 0, stream, nullptr, &act);
 }
 
 extern "C" int b200gnn_gemm_tf32x3_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,

@@ -31,7 +31,8 @@ constexpr int X_BOX = 8;                         // X lands as TM / X_BOX boxes 
 constexpr int RAW_BYTES = BKN * (TM + TN) * 4;   // 32 KB: X and G blocks as TMA lands them
 constexpr int OP_BYTES = 128 * BKN * 4;          // 16 KB: one transposed operand, [128 rows][32 nodes]
 constexpr int T_BYTES = 2 * OP_BYTES;            // G_hi, G_lo
-constexpr int SMEM_BYTES = STAGES * RAW_BYTES + 2 * T_BYTES + 256 + 1024;
+constexpr int SS_BYTES = TM / 2 * 16;             // ACT: {scale, shift} of the tile's column pairs (c, c + 8)
+constexpr int SMEM_BYTES = STAGES * RAW_BYTES + 2 * T_BYTES + 256 + SS_BYTES + 1024;
 constexpr int MAX_RANGES = 132;                  // node ranges (workspace partials): one CTA per SM over all tiles
 // The workspace holds at most the partials of the largest shape of the 128/256-wide layers (132 ranges of 256 x 256);
 // wider outputs have more tiles, fill the SMs with fewer ranges and get proportionally fewer partial slots.
@@ -43,8 +44,16 @@ struct Params {
   float* partial;   // [n_ranges][Kpad][Npad], Kpad = Kin rounded up to 128, Npad = Nout rounded up to 32 (TMA zero fill)
   int32_t Nn, Kin, Kpad, Nout, Npad, num_kb;
   int32_t n_tn, n_ranges;   // column tiles of dW, node ranges
+  // ACT: X is the BatchNorm input Y of a hidden layer and the operand is its activation, recomputed in registers from Y, the
+  // per-column scale / shift and the packed keep bits (uint32 [Nn][act_words]) exactly as gemm_tf32x3.cu's ACT prologue does
+  const float* act_scale;
+  const float* act_shift;
+  const uint32_t* act_bits;
+  int32_t act_words;
+  float inv_keep;
 };
 
+template <bool ACT>
 __global__ void __launch_bounds__(THREADS, 1)
 wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG, const Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -52,6 +61,7 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   uint8_t* tbuf = smem + STAGES * RAW_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(tbuf + 2 * T_BYTES);
   uint64_t* empty = full + STAGES;
+  float4* act_ss = reinterpret_cast<float4*>(tbuf + 2 * T_BYTES + 256);
 
   const int tiles = (p.Kpad / TM) * p.n_tn;
   const int tile = (int)blockIdx.x % tiles, range = (int)blockIdx.x / tiles;
@@ -89,13 +99,45 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   // X^T fragment of this thread: register i of k-step k is row (column of X) 64 cw + 16 (warp % 4) + lane / 4 + 8 (i % 2),
   // node 8 k + lane % 4 + 4 (i / 2), i.e. box 8 cw + 2 (warp % 4) + i % 2, column lane / 4 of the box
   const uint32_t xfrag = (8 * cw + 2 * (warp & 3)) * (BKN * X_BOX * 4) + (lane & 3) * (X_BOX * 4) + (lane >> 2) * 4;
+  // ACT: this thread's two X columns c0, c0 + 8 (one keep word: c0 % 32 < 24); their (scale, shift) wait in shared memory
+  // as act_ss[pair] = {sc(c0), sh(c0), sc(c0 + 8), sh(c0 + 8)}; lane l fetches the word of node 32 kb + l one block ahead,
+  // and the lanes that need it read it by shuffle
+  const int pair = cw * 32 + (warp & 3) * 8 + (lane >> 2);
+  const int c0 = mt * TM + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+  uint32_t wnext = 0u;
+  auto act_word = [&](int kb) {
+    const int node = kb * BKN + lane;
+    return node < p.Nn && (c0 >> 5) < p.act_words ? __ldg(p.act_bits + (size_t)node * p.act_words + (c0 >> 5)) : 0u;
+  };
+  if (ACT) {
+    if (ct < TM / 2) {
+      const int c = mt * TM + (ct >> 3) * 16 + (ct & 7);   // pair ct: columns c, c + 8
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (c < p.Kin) { v.x = __ldg(p.act_scale + c); v.y = __ldg(p.act_shift + c); }
+      if (c + 8 < p.Kin) { v.z = __ldg(p.act_scale + c + 8); v.w = __ldg(p.act_shift + c + 8); }
+      act_ss[ct] = v;
+    }
+    if (kb0 < kb1) wnext = act_word(kb0);
+    named_sync(1, 256);
+  }
   float acc[64], sum[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) sum[i] = acc[i] = 0.f;
   uint32_t xh0[BKN / 8][4], xl0[BKN / 8][4], xh1[BKN / 8][4], xl1[BKN / 8][4];   // X fragments of two consecutive blocks
   int s = 0; uint32_t ph = 0;
   auto block = [&](int i, uint32_t (&h)[BKN / 8][4], uint32_t (&l)[BKN / 8][4]) {
+    uint32_t wcur = 0u;
+    if (ACT) {
+      wcur = wnext;
+      if (kb0 + i + 1 < kb1) wnext = act_word(kb0 + i + 1);
+    }
     mbar_wait(&full[s], ph);
+    float4 ss = make_float4(0.f, 0.f, 0.f, 0.f);
+    int l4 = lane & 3;
+    if (ACT) {
+      ss = act_ss[pair];
+      asm volatile("" : "+r"(l4));             // shuffle source lanes formed per block, not held in 8 registers
+    }
     const uint32_t sraw = smem_u32(smem + s * RAW_BYTES);
     const float* rg = reinterpret_cast<const float*>(smem + s * RAW_BYTES + BKN * TM * 4);   // [32 nodes][128]
     uint8_t* T = tbuf + (i & 1) * T_BYTES;
@@ -116,8 +158,16 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
 #pragma unroll
     for (int k = 0; k < BKN / 8; ++k)
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        split1(lds32(sraw + xfrag + (j & 1) * (BKN * X_BOX * 4) + (8 * k + 4 * (j >> 1)) * (X_BOX * 4)), h[k][j], l[k][j]);
+      for (int j = 0; j < 4; ++j) {
+        // register j: column c0 + 8 (j % 2), node 8 k + lane % 4 + 4 (j / 2) of the block
+        uint32_t v = lds32(sraw + xfrag + (j & 1) * (BKN * X_BOX * 4) + (8 * k + 4 * (j >> 1)) * (X_BOX * 4));
+        if (ACT) {
+          const uint32_t w = __shfl_sync(0xffffffffu, wcur, 8 * k + l4 + 4 * (j >> 1));
+          const float y = fmaxf(fmaf(__uint_as_float(v), (j & 1) ? ss.z : ss.x, (j & 1) ? ss.w : ss.y), 0.f) * p.inv_keep;
+          v = (w >> ((c0 & 31) + 8 * (j & 1))) & 1u ? __float_as_uint(y) : 0u;
+        }
+        split1(v, h[k][j], l[k][j]);
+      }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     mbar_arrive(&empty[s]);                    // the raw block has been read
     if (i > 0) {                               // block i-1's wgmmas have retired: promote
@@ -226,8 +276,9 @@ extern "C" int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout) {
   return wgrad::range_cap(Kin, Nout) * wgrad::pad_k(Kin) * wgrad::pad_n(Nout);
 }
 
-extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW,
-                                             int64_t Nn, int64_t Kin, int64_t Nout, float* workspace, void* stream) {
+template <bool ACT>
+static int wgrad_launch(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW, int64_t Nn, int64_t Kin, int64_t Nout,
+                        float* workspace, const wgrad::Params& act, void* stream) {
   if (!X || !G || !dW || !workspace || Nn <= 0 || Kin <= 0 || Nout <= 0 || ldx < Kin || ldg < Nout || Nn >= INT32_MAX)
     return B200GNN_ERR_BAD_ARG;
   // tensor-core tiling: Kin a multiple of 4 up to 2048 (padded to 128), Nout a multiple of 4 up to 512 (padded to 32), both
@@ -242,14 +293,14 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const 
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad::wgrad_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(wgrad::wgrad_tf32x3_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          wgrad::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
     attr_set[dev] = true;
   }
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaStream_t st = (cudaStream_t)stream;
-  wgrad::Params p;
+  wgrad::Params p = act;
   p.partial = workspace; p.Nn = (int32_t)Nn; p.Kin = (int32_t)Kin; p.Nout = (int32_t)Nout;
   p.Kpad = (int32_t)wgrad::pad_k(Kin);
   p.Npad = (int32_t)wgrad::pad_n(Nout);
@@ -263,10 +314,27 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const 
   if (ranges < 1) ranges = 1;
   p.n_ranges = ranges;
   int rc;
-  wgrad::wgrad_tf32x3_kernel<<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
+  wgrad::wgrad_tf32x3_kernel<ACT><<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
   if ((rc = check_launch())) return rc;
   const int64_t n_vec = (int64_t)p.Kpad * p.Npad / 4;
   wgrad::wgrad_reduce_kernel<<<(int)((n_vec + wgrad::RED_VECS - 1) / wgrad::RED_VECS), wgrad::RED_VECS * wgrad::RED_GROUPS, 0, st>>>(
       reinterpret_cast<const float4*>(workspace), ranges, (int)Kin, p.Kpad, (int)Nout, p.Npad, dW);
   return check_launch();
+}
+
+extern "C" int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW,
+                                             int64_t Nn, int64_t Kin, int64_t Nout, float* workspace, void* stream) {
+  return wgrad_launch<false>(X, ldx, G, ldg, dW, Nn, Kin, Nout, workspace, wgrad::Params{}, stream);
+}
+
+// dW = act(Y)^T · G with act(Y) = dropout(relu(Y * scale + shift)) recomputed from Y and the packed keep bits
+// (uint32 [Nn][ceil(Kin / 32)], b200gnn_dropout_bits_u32): bit for bit the weight gradient of the materialised activation.
+extern "C" int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, const float* G, int64_t ldg, float* dW,
+                                                 int64_t Nn, int64_t Kin, int64_t Nout, const float* scale, const float* shift,
+                                                 const uint32_t* bits, float p_drop, float* workspace, void* stream) {
+  if (!scale || !shift || !bits || p_drop < 0.f || p_drop >= 1.f) return B200GNN_ERR_BAD_ARG;
+  wgrad::Params act{};
+  act.act_scale = scale; act.act_shift = shift; act.act_bits = bits; act.act_words = (int32_t)((Kin + 31) / 32);
+  act.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  return wgrad_launch<true>(Y, ldx, G, ldg, dW, Nn, Kin, Nout, workspace, act, stream);
 }

@@ -121,7 +121,8 @@ class ShardedGCNTrainer(GCNStudentTrainer):
         rowptr, col, val = shard_rows(rel, self.plan, self.rank)
         self._shard = csr_graph_from(rowptr, col, val, self.plan.real_rows(self.rank), self.plan.n_pad)
         self.n_global = adj.size(0)
-        super().__init__(adj, dims, _prebuilt_graph=self._shard, _rows_alloc=self.plan.block, **kw)
+        # this engine's forward / backward materialise the activations (fuse_activations is the single-GPU step's)
+        super().__init__(adj, dims, _prebuilt_graph=self._shard, _rows_alloc=self.plan.block, **{**kw, "fuse_activations": False})
         dev = self.device
         self.full = {k: torch.empty(self.plan.n_pad, k, device=dev) for k in set(dims[1:])}   # all-gather targets
         self.sum_buf = {k: torch.empty(2, k, device=dev) for k in set(dims[1:])}

@@ -5,7 +5,7 @@ Mirrors what one call of the reference's ``train()`` does for ``--gnn gcn --trai
 
     for each layer:  H = X W            (dense GEMM; cuBLAS fp32 through torch.mm — a plain library GEMM)
                      Y = Â H + b        (b200gnn SpMM, bias + BatchNorm statistics fused in the epilogue)
-                     X = dropout(relu(BN(Y)))   (one b200gnn pass)
+                     X = dropout(relu(BN(Y)))   (formed inside the GEMMs that read X, from Y and packed keep bits)
     loss, dlogits = fused CE/KD row kernel over logits[train_idx]
     backward: dH = Âᵀ dY (same SpMM kernel), dW = Xᵀ dH, dX = dH Wᵀ, fused BN/ReLU/dropout backward
     Adam over one flat parameter buffer.
@@ -53,7 +53,7 @@ class GCNStudentTrainer:
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
                  aggregate_first: Optional[bool] = None, tensor_core_gemm: bool = True, overlap_wgrad: bool = True,
-                 fuse_row_passes: bool = True, _prebuilt_graph: Optional[CsrGraph] = None, _rows_alloc: Optional[int] = None):
+                 fuse_row_passes: bool = True, fuse_activations: bool = True, _prebuilt_graph: Optional[CsrGraph] = None, _rows_alloc: Optional[int] = None):
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         self.device = adj.device
         self.dims, self.L = list(dims), len(dims) - 1
@@ -139,7 +139,7 @@ class GCNStudentTrainer:
             return blk[:N]
         self.H = [buf(dims[l + 1]) for l in range(self.L)]            # X W
         self.Y = [buf(dims[l + 1]) for l in range(self.L)]            # Â H + b  (last = logits)
-        self.A = [buf(dims[l + 1]) for l in range(self.L - 1)]        # dropout(relu(BN(Y)))
+        self._A = [buf(dims[l + 1]) for l in range(self.L - 1)]       # dropout(relu(BN(Y))): see the A property
         self.dY = [buf(dims[l + 1]) for l in range(self.L)]
         self.dH = [buf(dims[l + 1]) for l in range(self.L)]
         self.dA = [buf(dims[l + 1]) for l in range(self.L - 1)]
@@ -153,6 +153,20 @@ class GCNStudentTrainer:
         self.fuse_rows = bool(fuse_row_passes) and self.tc_gemm
         self._gemm_part = {k: torch.empty(ops.gemm_stat_slots(N, k), 2, k, device=dev)
                            for k in set(dims[1:-1]) if self.fuse_rows and ops.gemm_stats_supported(k)}
+        # Activations not materialised in training (the default where the fused kernels apply): the step draws the dropout
+        # keep decisions of all hidden layers as packed bits (one launch, on the side stream next to the layer-0
+        # aggregation), and every reader of A[l] (the next layer's GEMM, the weight-gradient GEMM, the BatchNorm-backward
+        # epilogue) recomputes it from Y[l], bn[l] scale / shift and the bits: the two [N, K] sweeps of the activation
+        # pass disappear.  The A property materialises the last training step's activations on first read.
+        hid = dims[1:-1]
+        self.fuse_act = (bool(fuse_activations) and self.fuse_rows and self.L >= 2 and len(set(hid)) == 1
+                         and ops.gemm_stats_supported(hid[0]) and hid[0] <= 2048
+                         and all(ops.wgrad_supported(dims[l], dims[l + 1]) for l in range(1, self.L)))
+        self.keep_bits = (torch.zeros(self.L - 1, N, (hid[0] + 31) // 32, dtype=torch.int32, device=dev)
+                          if self.fuse_act else None)
+        self._act_stale = False            # A[l] not yet materialised for the last forward
+        self._fwd_fused = False            # the last forward left its activations to the fused kernels
+        self._ev_bits = torch.cuda.Event()
         self.loss_out = self._grads_buf[self.n_par_pad:self.n_par_pad + 3]
         self.kd_part = torch.empty(2 * int(lib.load().b200gnn_kd_partials(N)), device=dev)
         self._graph = None
@@ -201,6 +215,19 @@ class GCNStudentTrainer:
                 self.running_mean[l].copy_(sd[f"bns.{l}.running_mean"]); self.running_var[l].copy_(sd[f"bns.{l}.running_var"])
 
     # ------------------------------------------------------------------ forward / backward
+    @property
+    def A(self) -> List[torch.Tensor]:
+        """Hidden activations dropout(relu(BN(Y))) of the last forward, [N, dims[l+1]] per hidden layer."""
+        if self._act_stale:
+            self._act_stale = False
+            for l in range(self.L - 1):
+                ops.affine_relu_bits(self.Y[l], self.keep_bits[l], self.bn[l][2], self.bn[l][3], self.p, out=self._A[l])
+        return self._A
+
+    def _act(self, l: int):
+        """(Y, scale, shift, keep bits) from which the fused kernels form hidden activation l."""
+        return self.Y[l], self.bn[l][2], self.bn[l][3], self.keep_bits[l]
+
     def activation_pattern(self, l: int) -> torch.Tensor:
         """bool [N, dims[l+1]]: ReLU-active AND kept by dropout in the last training forward of hidden layer l."""
         return self.A[l] > 0
@@ -214,6 +241,19 @@ class GCNStudentTrainer:
 
     def forward(self, x: torch.Tensor, training: bool = True) -> torch.Tensor:
         """Returns logits [N,C]; hidden activations stay in self.A (self.A[-1] is the reference's model.out_feat)."""
+        fused = training and self.fuse_act
+        self._act_stale = False
+        if fused:
+            # the keep bits need no input: drawn next to the first aggregation, joined before the first reader
+            if self._side is not None:
+                self._ev_fork.record(torch.cuda.current_stream())
+                self._side.wait_event(self._ev_fork)
+                with torch.cuda.stream(self._side):
+                    ops.dropout_bits(self.keep_bits, self.p, self.seed, 0, step_dev=self.step_count, step_mul=self.L)
+                self._ev_bits.record(self._side)
+            else:
+                ops.dropout_bits(self.keep_bits, self.p, self.seed, 0, step_dev=self.step_count, step_mul=self.L)
+        A = self._A
         inp = x
         for l in range(self.L):
             last = l == self.L - 1
@@ -230,38 +270,48 @@ class GCNStudentTrainer:
                         part = ops.col_stats(self.Y[0], partial=self._part(self.dims[1]))
                     ops.bn_finalize(part, self.N, self.gamma[0], self.beta[0], self.bn_eps,
                                     self.bn_momentum, self.running_mean[0], self.running_var[0], out=self.bn[0])
-                    ops.affine_relu_dropout(self.Y[0], self.bn[0][2], self.bn[0][3], True, self.p, self.seed, 0,
-                                            out=self.A[0], step_dev=self.step_count, step_mul=self.L)
+                    if not fused:
+                        ops.affine_relu_dropout(self.Y[0], self.bn[0][2], self.bn[0][3], True, self.p, self.seed, 0,
+                                                out=A[0], step_dev=self.step_count, step_mul=self.L)
                 else:
                     self._linear(0, self.AX, self.Y[0], bias=self.b[0])
                     scale = self.gamma[0] * torch.rsqrt(self.running_var[0] + self.bn_eps)
                     shift = self.beta[0] - self.running_mean[0] * scale
-                    ops.affine_relu_dropout(self.Y[0], scale, shift, True, 0.0, out=self.A[0])
-                inp = self.A[0]
+                    ops.affine_relu_dropout(self.Y[0], scale, shift, True, 0.0, out=A[0])
+                inp = A[0]
                 continue
-            self._linear(l, inp, self.H[l])
+            if fused and l > 0:
+                if l == 1 and self._side is not None:
+                    torch.cuda.current_stream().wait_event(self._ev_bits)
+                self._linear(l, None, self.H[l], act=self._act(l - 1))
+            else:
+                self._linear(l, inp, self.H[l])
             if last:
                 ops.spmm_csr(self.G, self.H[l], "sum", bias=self.b[l], out=self.Y[l])
             elif training:
                 ops.spmm_csr(self.G, self.H[l], "sum", bias=self.b[l], out=self.Y[l], stat_partial=self.stat_part[l])
                 ops.bn_finalize(self.stat_part[l], self.N, self.gamma[l], self.beta[l], self.bn_eps, self.bn_momentum,
                                 self.running_mean[l], self.running_var[l], out=self.bn[l])
-                ops.affine_relu_dropout(self.Y[l], self.bn[l][2], self.bn[l][3], True, self.p, self.seed, l,
-                                        out=self.A[l], step_dev=self.step_count, step_mul=self.L)
-                inp = self.A[l]
+                if not fused:
+                    ops.affine_relu_dropout(self.Y[l], self.bn[l][2], self.bn[l][3], True, self.p, self.seed, l,
+                                            out=A[l], step_dev=self.step_count, step_mul=self.L)
+                inp = A[l]
             else:
                 ops.spmm_csr(self.G, self.H[l], "sum", bias=self.b[l], out=self.Y[l])
                 scale = self.gamma[l] * torch.rsqrt(self.running_var[l] + self.bn_eps)
                 shift = self.beta[l] - self.running_mean[l] * scale
-                ops.affine_relu_dropout(self.Y[l], scale, shift, True, 0.0, out=self.A[l])
-                inp = self.A[l]
+                ops.affine_relu_dropout(self.Y[l], scale, shift, True, 0.0, out=A[l])
+                inp = A[l]
+        self._act_stale = self._fwd_fused = fused
         return self.Y[-1]
 
     def backward(self, x: torch.Tensor, d_out_feat: Optional[torch.Tensor] = None):
         """Consumes self.dY[-1] (d loss / d logits) and, for the auxiliary distillation losses, d loss / d out_feat
         ([N, H], added to the gradient arriving at the last hidden activation); fills self.grads."""
+        fused = self._fwd_fused
         for l in range(self.L - 1, -1, -1):
-            inp = x if l == 0 else self.A[l - 1]
+            act = self._act(l - 1) if fused and l > 0 else None
+            inp = x if l == 0 else (None if act else self._A[l - 1])
             if l == self.L - 1:
                 ops.col_sum(self.dY[l], out=self.gb[l], partial=self._part(self.dims[l + 1]))
             if l == 0 and self.agg_first:
@@ -279,11 +329,15 @@ class GCNStudentTrainer:
                     # dgrad GEMM whose epilogue masks by the ReLU/dropout pattern, stores dz and reduces the two BatchNorm
                     # backward column sums: pass 1 of the block's backward costs no sweep of its own
                     hi, lo = ops.split_tf32(self.W[l], transpose=False, hi=self.W_split[l][0], lo=self.W_split[l][1])
-                    ops.gemm_tf32x3_bnbwd(self.dH[l], hi, lo, d_prev, self.A[l - 1], self.Y[l - 1], self.bn[l - 1][0],
-                                          self.bn[l - 1][1], self.p, gp, accumulate=acc)
+                    if act:
+                        ops.gemm_tf32x3_bnbwd_bits(self.dH[l], hi, lo, d_prev, act[3], self.Y[l - 1], self.bn[l - 1][0],
+                                                   self.bn[l - 1][1], act[1], act[2], self.p, gp, accumulate=acc)
+                    else:
+                        ops.gemm_tf32x3_bnbwd(self.dH[l], hi, lo, d_prev, self._A[l - 1], self.Y[l - 1], self.bn[l - 1][0],
+                                              self.bn[l - 1][1], self.p, gp, accumulate=acc)
                 else:
                     self._linear_dgrad(l, self.dH[l], d_prev, accumulate=acc)
-            self._wgrad_async(l, inp, self.dH[l])                      # forks after the dgrad GEMM (both want the whole SM)
+            self._wgrad_async(l, inp, self.dH[l], act=act)             # forks after the dgrad GEMM (both want the whole SM)
             if l > 0:
                 k = self.dims[l]
                 part = self._part(k)
@@ -292,28 +346,32 @@ class GCNStudentTrainer:
                                          gp, self.N, self.p, self.dY[l - 1], self.ggamma[l - 1], self.gbeta[l - 1],
                                          self.gb[l - 1], part, self._coef(k))
                 else:
-                    ops.bn_act_bwd(d_prev, self.A[l - 1], self.Y[l - 1], self.bn[l - 1][0], self.bn[l - 1][1],
+                    ops.bn_act_bwd(d_prev, self._A[l - 1], self.Y[l - 1], self.bn[l - 1][0], self.bn[l - 1][1],
                                    self.gamma[l - 1], self.p, d_y=self.dY[l - 1], d_gamma=self.ggamma[l - 1],
                                    d_beta=self.gbeta[l - 1], d_bias=self.gb[l - 1], partial=part, coef=self._coef(k))
         self._wgrad_join()
 
-    def _wgrad_async(self, l: int, inp: torch.Tensor, d_out: torch.Tensor):
+    def _wgrad_async(self, l: int, inp: Optional[torch.Tensor], d_out: torch.Tensor, act=None):
         """grad W_l on the side stream, ordered after everything enqueued so far on the current stream."""
         if self._side is None:
-            return self._linear_wgrad(l, inp, d_out)
+            return self._linear_wgrad(l, inp, d_out, act)
         self._ev_fork.record(torch.cuda.current_stream())
         self._side.wait_event(self._ev_fork)
         with torch.cuda.stream(self._side):
-            self._linear_wgrad(l, inp, d_out)
+            self._linear_wgrad(l, inp, d_out, act)
 
     def _wgrad_join(self):
         if self._side is not None:
             self._ev_join.record(self._side)
             torch.cuda.current_stream().wait_event(self._ev_join)
 
-    def _linear(self, l: int, inp: torch.Tensor, out: torch.Tensor, bias: Optional[torch.Tensor] = None):
-        """out = inp @ W_l (+bias): wgmma 3xTF32 kernel, or cuBLAS fp32 when disabled."""
-        if self.tc_gemm:
+    def _linear(self, l: int, inp: Optional[torch.Tensor], out: torch.Tensor, bias: Optional[torch.Tensor] = None, act=None):
+        """out = inp @ W_l (+bias): wgmma 3xTF32 kernel, or cuBLAS fp32 when disabled.  act = (Y, scale, shift, bits): inp is
+        the activation formed from those inside the GEMM."""
+        if act is not None:
+            hi, lo = ops.split_tf32(self.W[l], transpose=True, hi=self.Wt_split[l][0], lo=self.Wt_split[l][1])
+            ops.gemm_tf32x3_act(*act, self.p, hi, lo, bias=bias, out=out)
+        elif self.tc_gemm:
             hi, lo = ops.split_tf32(self.W[l], transpose=True, hi=self.Wt_split[l][0], lo=self.Wt_split[l][1])
             ops.gemm_tf32x3(inp, hi, lo, bias=bias, out=out)
         elif bias is not None:
@@ -331,9 +389,11 @@ class GCNStudentTrainer:
         else:
             torch.mm(d_out, self.W[l].t(), out=d_inp)
 
-    def _linear_wgrad(self, l: int, inp: torch.Tensor, d_out: torch.Tensor):
-        """grad W_l = inp^T @ d_out: split-K wgmma kernel where the tiling allows, cuBLAS fp32 otherwise."""
-        if self.tc_gemm and ops.wgrad_supported(self.dims[l], self.dims[l + 1]):
+    def _linear_wgrad(self, l: int, inp: Optional[torch.Tensor], d_out: torch.Tensor, act=None):
+        """grad W_l = inp^T @ d_out: split-K wgmma kernel where the tiling allows, cuBLAS fp32 otherwise; act as in _linear."""
+        if act is not None:
+            ops.gemm_wgrad_tf32x3_act(*act, self.p, d_out, out=self.gW[l], workspace=self.wgrad_ws)
+        elif self.tc_gemm and ops.wgrad_supported(self.dims[l], self.dims[l + 1]):
             ops.gemm_wgrad_tf32x3(inp, d_out, out=self.gW[l], workspace=self.wgrad_ws)
         else:
             torch.mm(inp.t(), d_out, out=self.gW[l])
@@ -406,6 +466,7 @@ class GCNStudentTrainer:
 
     def replay(self, key: int = 0) -> torch.Tensor:
         self._graph[key].replay()
+        self._act_stale = self.fuse_act
         return self.loss_out
 
     # ------------------------------------------------------------------ accounting

@@ -238,7 +238,8 @@ class HybridGCNTrainer(GCNStudentTrainer):
         self._shard = csr_graph_from(rowptr, col, val, self.n_p, self.n_global)
         frp, fcol, fval = rel.csr()
         self.Gfull = csr_graph_from(frp, fcol, fval, self.n_global, self.n_global)
-        super().__init__(adj, dims, _prebuilt_graph=self._shard, _rows_alloc=self.plan.block, **kw)
+        # this engine's forward / backward materialise the activations (fuse_activations is the single-GPU step's)
+        super().__init__(adj, dims, _prebuilt_graph=self._shard, _rows_alloc=self.plan.block, **{**kw, "fuse_activations": False})
         dev = self.device
         N, L = self.n_global, self.L
         self.row0 = self.plan.offsets[self.rank]

@@ -56,6 +56,8 @@ SIGNATURES = {
     "b200gnn_affine_relu_dropout_scatter_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32p, _f32p, _int, _f32, _u64, _u64,
                                                        _i32p, _u64, _i32p, _u64, _i64, _i64, _ptr, _ptr, _i32, _i64, _ptr]),
     "b200gnn_dropout_mask_u8": (_int, [_ptr, _i64, _i64, _f32, _u64, _u64, _ptr]),
+    "b200gnn_dropout_bits_u32": (_int, [_ptr, _i64, _i64, _i64, _f32, _u64, _u64, _i32p, _u64, _ptr]),
+    "b200gnn_affine_relu_bits_f32": (_int, [_f32p, _ptr, _f32p, _f32p, _f32, _f32p, _i64, _i64, _ptr]),
     "b200gnn_relu_dropout_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _ptr]),
     "b200gnn_bn_act_bwd_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32, _f32p, _f32p,
                                       _f32p, _f32p, _f32p, _i64, _f32p, _ptr]),
@@ -78,11 +80,17 @@ SIGNATURES = {
                                              _ptr]),
     "b200gnn_gemm_tf32x3_bnbwd_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _int,
                                              _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _i64, _ptr]),
+    "b200gnn_gemm_tf32x3_bnbwd_bits_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _int,
+                                                  _ptr, _f32p, _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _i64, _ptr]),
+    "b200gnn_gemm_tf32x3_act_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p,
+                                           _f32p, _f32p, _ptr, _f32, _ptr]),
     "b200gnn_gemm_tf32x3_acc_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _ptr]),
     "b200gnn_gemm_tf32x3_scatter_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gemm_tf32x3_bcast_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_wgrad_workspace_floats": (_i64, [_i64, _i64]),
     "b200gnn_gemm_wgrad_tf32x3_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _ptr]),
+    "b200gnn_gemm_wgrad_tf32x3_act_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _f32p, _ptr, _f32,
+                                                 _f32p, _ptr]),
     "b200gnn_row_normalize_fwd_f32": (_int, [_f32p, _i64, _i64, _f32, _f32, _f32p, _f32p, _ptr]),
     "b200gnn_row_normalize_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _f32, _f32p, _int, _ptr]),
     "b200gnn_reduce_slots": (_i64, [_i64]),

@@ -209,6 +209,36 @@ def dropout_mask(n_rows: int, K: int, p: float, seed: int, offset: int, device="
     return mask
 
 
+def dropout_bits(bits: torch.Tensor, p: float, seed: int, offset: int, step_dev: Optional[torch.Tensor] = None,
+                 step_mul: int = 0, K: Optional[int] = None) -> torch.Tensor:
+    """Fill int32 bits[L, n, ceil(K/32)] with the keep decisions of affine_relu_dropout, one bit per element: layer l uses
+    offset + l (+ step_dev * step_mul).  K defaults to 32 * bits.shape[2]."""
+    n_layers, n, words = bits.shape
+    K = 32 * words if K is None else K
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and words == (K + 31) // 32
+    lib.check(lib.load().b200gnn_dropout_bits_u32(bits.data_ptr(), n_layers, n, K, p, seed, offset,
+                                                  lib.dptr(step_dev, torch.int32, "step_dev"), step_mul, lib.stream_ptr()),
+              "dropout_bits_u32")
+    return bits
+
+
+def _bits(bits: torch.Tensor, n: int, K: int) -> int:
+    if bits.dtype != torch.int32 or not bits.is_cuda or not bits.is_contiguous() or tuple(bits.shape) != (n, (K + 31) // 32):
+        raise lib.B200GnnError(f"keep bits: expected a contiguous CUDA int32 [{n}, {(K + 31) // 32}] tensor")
+    return bits.data_ptr()
+
+
+def affine_relu_bits(y: torch.Tensor, bits: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, p: float,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dropout(relu(y*scale + shift)) with the keep decisions of ``dropout_bits`` (bit-identical to affine_relu_dropout)."""
+    n, K = y.shape
+    if out is None:
+        out = torch.empty_like(y)
+    lib.check(lib.load().b200gnn_affine_relu_bits_f32(_f32(y, "y"), _bits(bits, n, K), _f32(scale, "scale"), _f32(shift, "shift"),
+                                                      p, _f32(out, "out"), n, K, lib.stream_ptr()), "affine_relu_bits_f32")
+    return out
+
+
 def bn_act_bwd(d_out, x_out, y, mean, invstd, gamma, p: float, d_y=None, d_gamma=None, d_beta=None, d_bias=None,
                partial=None, coef=None, want_dbias: bool = True):
     """Backward of x_out = dropout_p(relu(BN_train(y))). Returns (d_y, d_gamma, d_beta, d_bias)."""
@@ -331,6 +361,38 @@ def gemm_tf32x3_bnbwd(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, o
     return out
 
 
+def gemm_tf32x3_bnbwd_bits(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, out: torch.Tensor, bits: torch.Tensor,
+                           y: torch.Tensor, mean: torch.Tensor, invstd: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor,
+                           p: float, partial: torch.Tensor, accumulate: bool = False) -> torch.Tensor:
+    """gemm_tf32x3_bnbwd for an activation that is not materialised: [x_out > 0] is taken as bit && y*scale + shift > 0."""
+    M, K = a.shape
+    N = b_hi.shape[0]
+    assert out.shape == y.shape and out.stride(0) == y.stride(0)
+    lib.check(lib.load().b200gnn_gemm_tf32x3_bnbwd_bits_f32(_f32(a, "a"), a.stride(0), _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"),
+                                                            b_hi.stride(0), _f32(out, "out"), out.stride(0), M, N, K, int(accumulate),
+                                                            _bits(bits, M, N), _f32(y, "y"), _f32(mean, "mean"), _f32(invstd, "invstd"),
+                                                            _f32(scale, "scale"), _f32(shift, "shift"), float(p),
+                                                            _f32(partial, "partial"), partial.shape[0], lib.stream_ptr()),
+              "gemm_tf32x3_bnbwd_bits_f32")
+    return out
+
+
+def gemm_tf32x3_act(y: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, bits: torch.Tensor, p: float, b_hi: torch.Tensor,
+                    b_lo: torch.Tensor, bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = dropout(relu(y*scale + shift)) @ b^T (+bias), the activation formed in the GEMM's registers from y and the keep
+    bits of ``dropout_bits``: bit for bit gemm_tf32x3 of the materialised activation."""
+    M, K = y.shape
+    N = b_hi.shape[0]
+    assert b_hi.shape == b_lo.shape and b_hi.shape[1] == K
+    if out is None:
+        out = torch.empty(M, N, dtype=torch.float32, device=y.device)
+    lib.check(lib.load().b200gnn_gemm_tf32x3_act_f32(_f32(y, "y"), y.stride(0), _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"),
+                                                     b_hi.stride(0), _f32(out, "out"), out.stride(0), M, N, K, _f32(bias, "bias"),
+                                                     _f32(scale, "scale"), _f32(shift, "shift"), _bits(bits, M, K), float(p),
+                                                     lib.stream_ptr()), "gemm_tf32x3_act_f32")
+    return out
+
+
 def gemm_tf32x3_scatter(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, dst_ptrs, row_off: int,
                         bias: Optional[torch.Tensor] = None) -> None:
     """a[M,K] @ b[N,K]^T with column block q of the result stored to the [*, N/world] matrix at raw device address
@@ -391,6 +453,27 @@ def gemm_wgrad_tf32x3(x: torch.Tensor, g: torch.Tensor, out: Optional[torch.Tens
     lib.check(L.b200gnn_gemm_wgrad_tf32x3_f32(_f32(x, "x"), x.stride(0), _f32(g, "g"), g.stride(0), _f32(out, "out"), nn_,
                                               k_in, n_out, _f32(workspace, "workspace"), lib.stream_ptr()),
               "gemm_wgrad_tf32x3_f32")
+    return out
+
+
+def gemm_wgrad_tf32x3_act(y: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, bits: torch.Tensor, p: float,
+                          g: torch.Tensor, out: Optional[torch.Tensor] = None,
+                          workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemm_wgrad_tf32x3 of x = dropout(relu(y*scale + shift)), x formed in registers from y and the keep bits."""
+    nn_, k_in = y.shape
+    n_out = g.shape[1]
+    assert g.shape[0] == nn_
+    if not wgrad_supported(k_in, n_out):
+        raise lib.B200GnnError(f"gemm_wgrad_tf32x3_act: Kin={k_in}, Nout={n_out} is outside the 128/256-row tilings")
+    L = lib.load()
+    if out is None:
+        out = torch.empty(k_in, n_out, dtype=torch.float32, device=y.device)
+    if workspace is None:
+        workspace = torch.empty(int(L.b200gnn_wgrad_workspace_floats(k_in, n_out)), dtype=torch.float32, device=y.device)
+    lib.check(L.b200gnn_gemm_wgrad_tf32x3_act_f32(_f32(y, "y"), y.stride(0), _f32(g, "g"), g.stride(0), _f32(out, "out"), nn_,
+                                                  k_in, n_out, _f32(scale, "scale"), _f32(shift, "shift"), _bits(bits, nn_, k_in),
+                                                  float(p), _f32(workspace, "workspace"), lib.stream_ptr()),
+              "gemm_wgrad_tf32x3_act_f32")
     return out
 
 

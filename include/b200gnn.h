@@ -187,6 +187,16 @@ int b200gnn_affine_relu_dropout_scatter_f32(const float* Y, float* out, int64_t 
                                             const int32_t* row_off, int32_t world, int64_t ld_dst, void* stream);
 int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K, float p,
                             uint64_t seed, uint64_t offset, void* stream);
+/* The keep decisions of b200gnn_affine_relu_dropout_f32 (row_offset 0) packed one bit per element, for n_layers
+ * [n_rows, K] activations in one launch: layer l uses effective offset offset + l (+ *step_dev * step_mul) and fills
+ * bits[l][row][w], w < ceil(K/32), bit b = column 32 w + b (bits past K are zero).  Needs no input: it can run next to
+ * whatever precedes the first consumer.  The fused GEMMs (_act / _bits entry points) recompute the activation from Y,
+ * scale / shift and these bits; b200gnn_affine_relu_bits_f32 materialises it (bit-identical to
+ * b200gnn_affine_relu_dropout_f32 with relu = 1 for the same decisions). */
+int b200gnn_dropout_bits_u32(uint32_t* bits, int64_t n_layers, int64_t n_rows, int64_t K, float p, uint64_t seed,
+                             uint64_t offset, const int32_t* step_dev, uint64_t step_mul, void* stream);
+int b200gnn_affine_relu_bits_f32(const float* Y, const uint32_t* bits, const float* scale, const float* shift,
+                                 float p, float* out, int64_t n_rows, int64_t K, void* stream);
 /* Backward of out = dropout_p(relu(Y)) (no BatchNorm): dY = dOut * [Xout > 0] / (1-p), contiguous [n_rows, K]
  * rows, K a multiple of 4; dY may alias dOut. */
 int b200gnn_relu_dropout_bwd_f32(const float* dOut, const float* Xout, float* dY,
@@ -296,6 +306,20 @@ int b200gnn_gemm_tf32x3_bnbwd_f32(const float* A, int64_t lda, const float* B_hi
                                   float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
                                   const float* Xout, const float* Y, const float* mean, const float* invstd, float p_drop,
                                   float* partial, int64_t slots, void* stream);
+/* Activations that are not materialised: Xout = dropout(relu(Y*scale + shift)) is recomputed from Y, the BatchNorm's
+ * scale / shift and the packed keep bits of b200gnn_dropout_bits_u32 (uint32 [rows][ceil(width/32)]).
+ *   _bnbwd_bits_f32 : _bnbwd_f32 with the mask [Xout > 0] taken as bit && Y*scale + shift > 0 (bits of the N columns).
+ *   _act_f32        : C = Xout · B^T (+ bias) with Xout formed from Y = A in the GEMM's registers, bit for bit the
+ *                     product of the materialised activation (bits of the K columns; K <= 2048). */
+int b200gnn_gemm_tf32x3_bnbwd_bits_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                       float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
+                                       const uint32_t* bits, const float* Y, const float* mean, const float* invstd,
+                                       const float* scale, const float* shift, float p_drop, float* partial,
+                                       int64_t slots, void* stream);
+int b200gnn_gemm_tf32x3_act_f32(const float* Y, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                const float* scale, const float* shift, const uint32_t* bits, float p_drop,
+                                void* stream);
 /* Same GEMM with the R->C layout exchange of the multi-GPU engine fused into the epilogue: output columns
  * [q*kc, (q+1)*kc), kc = N/world (a multiple of 32), are stored to C_ptrs[q][(row_off + m)*kc + ...] — C_ptrs is a HOST array
  * of `world` device pointers (the ranks' [N_nodes, kc] buffers, peer-mapped), so the tile results cross NVLink as they are
@@ -319,6 +343,10 @@ int b200gnn_gemm_wgrad_tf32x3_f32(const float* X, int64_t ldx, const float* G,
                                   int64_t ldg, float* dW, int64_t Nn,
                                   int64_t Kin, int64_t Nout, float* workspace,
                                   void* stream);
+/* ... with X = dropout(relu(Y*scale + shift)) recomputed from Y and the packed keep bits (uint32 [Nn][ceil(Kin/32)]). */
+int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, const float* G, int64_t ldg, float* dW,
+                                      int64_t Nn, int64_t Kin, int64_t Nout, const float* scale, const float* shift,
+                                      const uint32_t* bits, float p_drop, float* workspace, void* stream);
 
 /* ------------------------------------------------------------------ *
  * Feature-distillation criteria (arxiv_pyg/criterion.py): row / pair passes.
