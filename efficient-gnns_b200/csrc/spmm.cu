@@ -708,6 +708,230 @@ __global__ void __launch_bounds__(SPMM_THREADS, 3) spmm_rows_bulk_kernel(const S
 }
 
 
+// ------------------------------------------------------------------ lane-copy column-slab kernel (K = 128 or 256, X beyond L2)
+// When X is larger than L2, the bulk kernel's 128- or 256-float slabs (87 / 173 MB at ARXIV shape) still come mostly from
+// DRAM.  This kernel tiles K into narrow slabs of SW floats (SLAB_SW = 64), so the [N, SW] operand of one slab (43 MB at
+// N = 169,343) mostly stays in L2 while the resident CTAs gather from it; DRAM then carries X about once, Y once and
+// (col, val) once per slab.  A narrow row is too small for one bulk copy each (the copy engine retires a roughly fixed
+// number of copies per second), so the lanes issue the copies: every lane copies 16-byte slices with cp.async.cg into a
+// per-warp ring, E = 32·4 / SW neighbour rows per warp instruction, SLAB_G rows per commit group, the ring keeping about
+// 6 KB per warp in flight across row boundaries.  A slice is consumed by another lane than the one that copied it, so
+// cp.async.wait_group is followed by __syncwarp() before the reads, and the reads by __syncwarp() before the refill.
+// The slab gathers carry an evict_last L2 policy; (col, val) are loaded evict_first and Y is stored st.global.cs (when
+// stream_store), so the index and output streams do not push the slab out of L2.
+// Arithmetic: lane l owns floats [l·SW/32, (l+1)·SW/32) of the slab and forms acc = fmaf(w_e, x_e, acc) from zero in CSR
+// edge order, then the bulk kernel's epilogue (/ max(deg, 1), + bias, store, statistics) and its warp-ordered statistics
+// combine: every Y element and statistics slot equals spmm_rows_bulk_kernel's bit for bit.  Hub rows take
+// spmm_hub_seg_cta over the full width in the CTAs that lead the grid, whose per-element order is the bulk path's too.
+constexpr int SLAB_RING = 8192;                  // ring bytes per warp
+constexpr int SLAB_G = 8;                        // neighbour rows per cp.async group
+constexpr int SLAB_SMEM = SPMM_WARPS * SLAB_RING;
+
+__device__ __forceinline__ void cp_async16_pol(void* smem_dst, const void* gsrc, uint64_t pol) {
+  asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ int32_t ldg_pol(const int32_t* p, uint64_t pol) {
+  int32_t v;
+  asm("ld.global.nc.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ float ldg_pol(const float* p, uint64_t pol) {
+  float v;
+  asm("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+  return v;
+}
+
+template <int SW> struct SlabLane;               // a lane's share of one slab row
+template <> struct SlabLane<32> { using V = float; };
+template <> struct SlabLane<64> { using V = float2; };
+
+template <int SW, bool HAS_VAL, bool STATS>
+__device__ __forceinline__ void spmm_chunk_cta_slab(const SpmmParams& p, const int cta, const int slab, float* s_stat,
+                                                    float* ring_all) {
+  using V = typename SlabLane<SW>::V;
+  constexpr int LPR = SW / 4;                     // lanes per neighbour row (16 B each)
+  constexpr int E = 32 / LPR;                     // neighbour rows per warp-wide cp.async
+  constexpr int D = SLAB_RING / (SW * 4);         // ring depth in neighbour rows
+  constexpr int G = SLAB_G, NG = D / G;           // commit groups in the ring
+  static_assert(G % E == 0 && 32 % G == 0 && NG >= 2 && (D & (D - 1)) == 0, "ring geometry");
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* ring = ring_all + (size_t)warp * (SLAB_RING / 4);   // slot s: ring[s*SW .. s*SW + SW)
+  uint64_t pol_keep, pol_stream;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_keep));
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_stream));
+
+  const int f0 = slab * SW;
+  const float* Xs = p.X + f0 + (lane % LPR) * 4;  // this lane's 16-byte slice of a neighbour's slab row
+  float* ring_dst = ring + (lane / LPR) * SW + (lane % LPR) * 4;
+  const int vlane = slab * 32 + lane;             // this lane's V index within a row of Y / bias
+
+  V ssum, ssq, bias_l;
+  vzero(ssum); vzero(ssq); vzero(bias_l);
+  if (p.bias) bias_l = load_bias<V>(p.bias, vlane);
+
+  const int chunk = cta * SPMM_WARPS + warp;
+  const int row_lo = chunk < p.n_chunks ? __ldg(p.chunk_rowptr + chunk) : 0;
+  const int row_hi = chunk < p.n_chunks ? __ldg(p.chunk_rowptr + chunk + 1) : 0;
+
+  auto flush = [&](int row, int deg, V& acc) {
+    V y = acc;
+    if (p.mean) vdiv(y, (float)max(deg, 1));
+    vadd(y, bias_l);
+    V* dst = reinterpret_cast<V*>(p.Y + (size_t)row * p.ldy) + vlane;
+    if (p.stream_store) vstcs(dst, y); else *dst = y;
+    if (STATS) vstat(ssum, ssq, y);
+    vzero(acc);
+  };
+
+  int next_r = row_lo, next_e = row_lo < row_hi ? __ldg(p.rowptr + row_lo) : 0;
+  for (int r = row_lo, e_r = next_e; r < row_hi; r = next_r, e_r = next_e) {
+    // ---- a run [r, run_end) of consecutive non-hub rows, ended by a hub row (which belongs to the split path) or by the
+    // chunk's end.  A chunk is a few rows and this kernel walks every chunk once per slab, so the run is found 32 rows at a
+    // time (one load and a ballot over the degrees) rather than with one dependent rowptr load per row.
+    const int e_lo = e_r;
+    int run_end = r, e_hi = e_r, rp_first = 0;
+    for (;;) {
+      const int rr = run_end + lane;
+      const int rp1 = rr < row_hi ? __ldg(p.rowptr + rr + 1) : 0;
+      if (run_end == r) rp_first = rp1;           // rowptr[r + lane + 1]: the run's first 32 row ends
+      int rp0 = __shfl_up_sync(FULL_MASK, rp1, 1);
+      if (lane == 0) rp0 = e_hi;
+      const unsigned stop = __ballot_sync(FULL_MASK, rr >= row_hi || rp1 - rp0 > p.hub_threshold);
+      const int k = stop ? __ffs(stop) - 1 : 31;
+      const int end_before = __shfl_sync(FULL_MASK, rp1, (k + 31) & 31);   // rowptr[run_end + k] when k > 0
+      next_e = __shfl_sync(FULL_MASK, rp1, k);                            // rowptr[run_end + k + 1]
+      if (stop) {
+        if (k > 0) e_hi = end_before;
+        run_end += k;
+        break;
+      }
+      e_hi = next_e;
+      run_end += 32;
+    }
+    next_r = run_end + 1;                         // past the hub row that ends the run (or past row_hi)
+    if (run_end == r) continue;                   // row r is a hub row
+    const int n = e_hi - e_lo;
+
+    // Edge windows of 32 (col, val), each loaded one window ahead of its use so that the load latency hides behind the
+    // previous window's gathers; the first two are loaded here, before the run's first copies and empty rows.
+    auto col_win = [&](int jw) { const int e = e_lo + jw + lane; return e < e_hi ? ldg_pol(p.col + e, pol_stream) : 0; };
+    auto val_win = [&](int jw) { const int e = e_lo + jw + lane; return e < e_hi ? ldg_pol(p.val + e, pol_stream) : 0.f; };
+    int cI = col_win(0), cN = col_win(32);
+    float vA = 1.f, vN = 1.f;
+    if (HAS_VAL) { vA = val_win(0); vN = val_win(32); }
+
+    int rbase = r;                                // row ends of the run, 32 at a time in registers
+    int rp = (rbase + lane < run_end) ? rp_first : e_hi;
+    auto row_end_of = [&](int row) {
+      if (row - rbase >= 32) {                    // warp-uniform
+        rbase = row;
+        rp = (rbase + lane < run_end) ? __ldg(p.rowptr + rbase + lane + 1) : e_hi;
+      }
+      return __shfl_sync(FULL_MASK, rp, row - rbase);
+    };
+
+    V acc;
+    vzero(acc);
+    int row_beg = e_lo;
+    int rend = row_end_of(r);
+    while (r < run_end && rend == row_beg) {      // leading empty rows
+      flush(r, 0, acc);
+      ++r;
+      if (r < run_end) rend = row_end_of(r);
+    }
+    if (n == 0) continue;
+
+    // Issue side: the column window (cI); edge jg + u is copied by lanes [u%E·LPR, u%E·LPR + LPR) of warp instruction u/E.
+    // Consume side: the value window (vA).  Both advance in groups of G edges; one commit per group (empty past the run's
+    // end, so the group count stays uniform), NG groups in the ring.
+    auto issue_group = [&](int jg, int slot0) {   // edges jg..jg+G-1 (relative to e_lo) -> slots slot0..slot0+G-1
+      if (jg < n) {                               // warp-uniform
+        if (jg > 0 && (jg & 31) == 0) { cI = cN; cN = col_win(jg + 32); }
+#pragma unroll
+        for (int i = 0; i < G / E; ++i) {
+          const int u = i * E + lane / LPR;
+          const int cc = __shfl_sync(FULL_MASK, cI, (jg + u) & 31);
+          if (jg + u < n) cp_async16_pol(ring_dst + (slot0 + i * E) * SW, Xs + (size_t)cc * p.ldx, pol_keep);
+        }
+      }
+      cp_async_commit();
+    };
+    auto boundary = [&]() {                       // the current row is complete: store it (+ empty rows that follow)
+      do {
+        flush(r, rend - row_beg, acc);
+        row_beg = rend;
+        ++r;
+        if (r < run_end) rend = row_end_of(r);
+      } while (r < run_end && rend == row_beg);
+    };
+    auto consume_group = [&](int j0, int slot0) {  // j0 < n
+      if (HAS_VAL && j0 > 0 && (j0 & 31) == 0) { vA = vN; vN = val_win(j0 + 32); }
+      const V* sbase = reinterpret_cast<const V*>(ring + slot0 * SW) + lane;
+      const int cnt = min(G, n - j0);
+      int done = 0;
+      while (done < cnt) {                        // pieces of the group that lie in one row (all warp-uniform)
+        const int room = rend - (e_lo + j0 + done);   // >= 1: edges left in the current row
+        const int take = min(cnt - done, room);
+        if (take == G) {                          // common case: the whole group inside one row
+#pragma unroll
+          for (int u = 0; u < G; ++u) {
+            const float w = HAS_VAL ? __shfl_sync(FULL_MASK, vA, (j0 + u) & 31) : 1.f;
+            vfma(acc, w, sbase[u * 32]);
+          }
+        } else {
+#pragma unroll 1
+          for (int u = done; u < done + take; ++u) {
+            const float w = HAS_VAL ? __shfl_sync(FULL_MASK, vA, (j0 + u) & 31) : 1.f;
+            vfma(acc, w, sbase[u * 32]);
+          }
+        }
+        done += take;
+        if (take == room) boundary();
+      }
+    };
+#pragma unroll
+    for (int g = 0; g < NG; ++g) issue_group(g * G, g * G);
+#pragma unroll 1
+    for (int j = 0, s0 = 0; j < n; j += G, s0 = (s0 + G) & (D - 1)) {
+      cp_async_wait<NG - 1>();                    // this thread's copies of the oldest group have landed
+      __syncwarp();                               // ... and every other lane's
+      consume_group(j, s0);
+      __syncwarp();                               // every lane has read the slots before they are refilled
+      issue_group(j + D, s0);
+    }
+    cp_async_wait<0>();
+  }
+
+  if (STATS) {
+    float* ss = s_stat;
+    float* sq = s_stat + SW;
+    for (int i = threadIdx.x; i < 2 * SW; i += SPMM_THREADS) s_stat[i] = 0.f;
+    __syncthreads();
+    for (int w = 0; w < SPMM_WARPS; ++w) {          // fixed order => deterministic, the bulk kernel's order
+      if (warp == w) smem_accum(ss, sq, lane, ssum, ssq);
+      __syncthreads();
+    }
+    float* out = p.stat_partial + (size_t)cta * 2 * p.K + f0;
+    for (int i = threadIdx.x; i < SW; i += SPMM_THREADS) { out[i] = ss[i]; out[p.K + i] = sq[i]; }
+  }
+}
+
+// Grid: the n_seg hub-segment CTAs (full width), then n_slabs slabs of main_grid chunk CTAs each, slab-major.
+template <int SW, bool HAS_VAL, bool STATS>
+__global__ void __launch_bounds__(SPMM_THREADS, 3) spmm_rows_slab_kernel(const SpmmParams p) {
+  __shared__ float s_mem[2 * SPMM_MAX_SLAB_FLOATS];
+  extern __shared__ __align__(128) unsigned char s_dyn[];
+  const int b = (int)blockIdx.x;
+  if (b < p.n_seg) {   // CH = 1: 128-float passes; each element's order does not depend on CH (and CH = 2 would spill)
+    spmm_hub_seg_cta<float4, 1, HAS_VAL>(p, b, s_mem);
+    return;
+  }
+  const int slab = (b - p.n_seg) / p.main_grid;
+  spmm_chunk_cta_slab<SW, HAS_VAL, STATS>(p, b - p.n_seg - slab * p.main_grid, slab, s_mem, reinterpret_cast<float*>(s_dyn));
+}
+
+
 // ------------------------------------------------------------------ narrow rows (K <= 64 floats: e.g. the 40 logits)
 // A 160-byte row needs only 10 lanes.  Instead of folding several NEIGHBOURS of one row across the warp (which drains
 // at every row end and needs cross-group shuffles), each group of lanes takes its OWN ROW of the chunk: 3 rows
@@ -931,6 +1155,36 @@ static int launch_spmm_bulk(const SpmmParams& p, cudaStream_t st, bool two_ctas)
   return B200GNN_OK;
 }
 
+template <int SW>
+static int launch_spmm_slab(const SpmmParams& p, cudaStream_t st) {
+  int rc;
+  const bool stats = p.stat_partial != nullptr;
+  const int grid = p.n_seg + p.main_grid * p.n_slabs;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static bool attr_done[64] = {};                  // per device (cudaFuncSetAttribute is per device); idempotent if raced
+  if (dev >= 0 && dev < 64 && !attr_done[dev]) {
+    cudaFuncSetAttribute(spmm_rows_slab_kernel<SW, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SLAB_SMEM);
+    cudaFuncSetAttribute(spmm_rows_slab_kernel<SW, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SLAB_SMEM);
+    cudaFuncSetAttribute(spmm_rows_slab_kernel<SW, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SLAB_SMEM);
+    cudaFuncSetAttribute(spmm_rows_slab_kernel<SW, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SLAB_SMEM);
+    attr_done[dev] = true;
+  }
+  if (p.val) {
+    if (stats) spmm_rows_slab_kernel<SW, true, true><<<grid, SPMM_THREADS, SLAB_SMEM, st>>>(p);
+    else spmm_rows_slab_kernel<SW, true, false><<<grid, SPMM_THREADS, SLAB_SMEM, st>>>(p);
+  } else {
+    if (stats) spmm_rows_slab_kernel<SW, false, true><<<grid, SPMM_THREADS, SLAB_SMEM, st>>>(p);
+    else spmm_rows_slab_kernel<SW, false, false><<<grid, SPMM_THREADS, SLAB_SMEM, st>>>(p);
+  }
+  if ((rc = check_launch())) return rc;
+  if (p.n_hub > 0) {
+    spmm_hub_finalize_kernel<<<p.n_hub, 256, 0, st>>>(p);
+    if ((rc = check_launch())) return rc;
+  }
+  return B200GNN_OK;
+}
+
 template <typename V>
 static int dispatch_ch(const SpmmParams& p, cudaStream_t st) {
   if (p.nvec <= 32) return launch_spmm<V, 1>(p, st);
@@ -1037,6 +1291,13 @@ static int bulk_auto_slab(int64_t K, int64_t n_src) {
   (void)n_src;
   return (K % 256 == 0) ? 256 : 128;
 }
+// The lane-copy slab kernel takes K = 128 / 256 when X is larger than SLAB_L2_BUDGET bytes and the choice is automatic.
+// tools/l2_probe.cu (H100 SXM, BENCH.md): random 256-byte row gathers reach 7.3 TB/s from tables up to 40 MB, 6.7 at
+// 48 MB, 5.7 at 64 MB; below 40 MB the bulk kernel's full-width rows are L2 hits already.  Slab width 64 floats: 32-float
+// slabs (22 MB per slab at ARXIV shape) hit L2 more often but double the per-slab walk of every chunk, and measured
+// slower than the bulk kernel at both widths.
+constexpr int64_t SLAB_L2_BUDGET = (int64_t)40 << 20;
+constexpr int SLAB_SW = 64;
 extern "C" void b200gnn_spmm_set_variant(int v) { g_spmm_variant = v; }
 
 extern "C" int64_t b200gnn_csr_chunk_count(int64_t n_rows, int64_t nnz, int32_t chunk_nnz, int32_t row_cost) {
@@ -1127,6 +1388,13 @@ extern "C" int b200gnn_spmm_csr_f32(const int32_t* rowptr, const int32_t* col, c
   //   per pass, 4 bulk-copy ring with 128-float slabs, 5 bulk-copy ring with 256-float slabs, 6 / 7 bulk-copy ring
   //   with 128-float slabs and 8 / 4 edges per barrier group;
   //   +16 = evict_last L2 policy on the gathers, +32 = the other barrier-group size, +64 = 2 CTAs per SM.
+  // Automatic choice only: X beyond the L2 budget at the widths the bulk kernel serves -> the lane-copy slab kernel,
+  // which reproduces the bulk kernel's results bit for bit.
+  if (g_spmm_variant == 0 && W == 4 && p.n_yp == 0 && (K == 128 || K == 256) && n_src * K * 4 > SLAB_L2_BUDGET) {
+    p.n_slabs = (int32_t)(K / SLAB_SW);
+    return launch_spmm_slab<SLAB_SW>(p, st);
+  }
+
   const int fam = g_spmm_variant & 15;
   const bool alt_g = (g_spmm_variant & 32) != 0;
   int bulk_sw = 0;                                  // slab width in floats (0 = not the bulk kernel)
