@@ -131,16 +131,6 @@ __device__ __forceinline__ float4 affine_relu4(float4 y, const float* __restrict
   if (relu) { y.x = fmaxf(y.x, 0.f); y.y = fmaxf(y.y, 0.f); y.z = fmaxf(y.z, 0.f); y.w = fmaxf(y.w, 0.f); }
   return y;
 }
-__device__ __forceinline__ uchar4 keep16(uint32_t a, uint32_t b, uint32_t thr) {
-  uchar4 m;
-  m.x = (a & 0xffffu) >= thr; m.y = (a >> 16) >= thr; m.z = (b & 0xffffu) >= thr; m.w = (b >> 16) >= thr;
-  return m;
-}
-__device__ __forceinline__ uchar4 keep24(const uint4& r, float p) {
-  uchar4 m;
-  m.x = u32_to_unit(r.x) >= p; m.y = u32_to_unit(r.y) >= p; m.z = u32_to_unit(r.z) >= p; m.w = u32_to_unit(r.w) >= p;
-  return m;
-}
 
 template <bool P16>
 __global__ void __launch_bounds__(256) affine_relu_dropout_kernel(const float* __restrict__ Y, float* __restrict__ out,
@@ -320,13 +310,6 @@ __global__ void __launch_bounds__(256) affine_relu_bits_kernel(const float* __re
     y.z = (b & 4u) ? y.z * inv_keep : 0.f; y.w = (b & 8u) ? y.w * inv_keep : 0.f;
     st4(out + 4 * i, y);
   }
-}
-
-// p * 65536 integral (and p > 0): the 16-bit decision path is exact
-static inline bool dropout_p16(float p, uint32_t& thr16) {
-  const double t = (double)p * 65536.0;
-  thr16 = (uint32_t)t;
-  return p > 0.f && t == (double)thr16;
 }
 
 // ---------------------------------------------------------------- backward of ReLU+dropout (no BatchNorm)

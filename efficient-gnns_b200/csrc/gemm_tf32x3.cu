@@ -120,6 +120,14 @@ struct Params {
   const float* act_shift;
   const uint32_t* act_bits;
   int32_t act_words;
+  // PRELU (SIGN's FeedForwardNet): A = dropout(prelu(Z)) with one learnable slope read from device memory, so no per-column
+  // table and no limit on K:
+  //   stat_mode 0: every A fragment element z becomes bit ? (z > 0 ? z : slope * z) * inv_keep : 0 before its tf32 split;
+  //   stat_mode 4: C is dA, the gradient of that activation over N columns (Z = bn_y, pitch ldc, bits [M][act_words]): the
+  //                epilogue STORES dz = (bit ? dA * inv_keep : 0) * (z > 0 ? 1 : slope) and reduces the slope gradient
+  //                sum (bit ? dA * inv_keep : 0) * z over z <= 0 in fp64 into slope_partial[cta * 8 + warp] (fixed order).
+  const float* act_slope;
+  double* slope_partial;
 };
 
 // stat_mode 2: the pieces of Xout / Y one lane needs for a 32-column chunk (4 rows x 4 columns: rows it*4 + lane/8
@@ -154,16 +162,26 @@ __device__ __forceinline__ uint32_t act1(uint32_t y, float sc, float sh, uint32_
   return keep ? __float_as_uint(fmaxf(fmaf(__uint_as_float(y), sc, sh), 0.f) * inv_keep) : 0u;
 }
 
-// STAT: 0 plain, 1 / 2 the fused column reductions (Params::stat_mode); PEER: the output goes to peer buffers (Params::Cp);
-// ACT: the hidden activation is recomputed from Y (Params::act_bits).  Compile-time so that each instantiation carries only
-// its own prologue and epilogue (the epilogue is the hot loop of the narrow-K GEMMs).
-template <class C, int STAT, bool PEER, bool ACT = false>
+// PReLU + dropout of one A element z (SIGN): the same operations as b200gnn_prelu_bits_f32
+__device__ __forceinline__ uint32_t prelu1(uint32_t z, float slope, uint32_t keep, float inv_keep) {
+  const float x = __uint_as_float(z);
+  return keep ? __float_as_uint((x > 0.f ? x : slope * x) * inv_keep) : 0u;
+}
+
+// STAT: 0 plain, 1 / 2 the fused column reductions (Params::stat_mode), 4 the PReLU/dropout backward; PEER: the output goes
+// to peer buffers (Params::Cp); ACT: the hidden activation is recomputed from Y (Params::act_bits); PRELU: the PReLU/dropout
+// prologue.  Compile-time so that each instantiation carries only its own prologue and epilogue (the epilogue is the hot loop
+// of the narrow-K GEMMs).
+template <class C, int STAT, bool PEER, bool ACT = false, bool PRELU = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                    const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmX,
                    const __grid_constant__ CUtensorMap tmY, const Params p) {
-  constexpr bool BNB = STAT >= 2;        // BatchNorm-backward epilogue; STAT == 3: its Xout / Y blocks arrive by TMA
+  constexpr bool BNB = STAT == 2 || STAT == 3;   // BatchNorm-backward epilogue; STAT == 3: its Xout / Y blocks arrive by TMA
   constexpr bool XYTMA = STAT == 3;
+  constexpr bool COLSTAT = STAT >= 1 && STAT <= 3;   // per-column reductions in the statistics block
+  constexpr bool PRB = STAT == 4;                    // PReLU/dropout backward epilogue
+  constexpr bool PRO = (ACT || PRELU) && !STAT;      // activation prologue on A (keep words fetched a stage ahead)
   constexpr int BN = C::BN, STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, B_TILE_BYTES = C::B_TILE_BYTES, ACC = C::ACC;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -215,7 +233,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const int q = warp - 4;                         // consumer warp: rows [16 q, 16 q + 16)
   const bool vec_ok = PEER ? true : ((p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0));
   float* stat = stat_smem + q * (2 * STAT_MAX_N);  // this warp's [2][N] column accumulators
-  if (STAT) {
+  if (COLSTAT) {
     for (int i = lane; i < 2 * p.N; i += 32) stat[i] = 0.f;
     __syncwarp();
   }
@@ -259,7 +277,9 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     w[1] = r + 8 < p.M ? __ldg(p.act_bits + (size_t)(r + 8) * p.act_words + kb) : 0u;
   };
   uint32_t wnext[2] = {0u, 0u};
-  if (ACT && !STAT && blockIdx.x < num_tiles) act_words(blockIdx.x, 0, wnext);
+  if (PRO && blockIdx.x < num_tiles) act_words(blockIdx.x, 0, wnext);
+  const float slope = (PRELU || PRB) ? __ldg(p.act_slope) : 0.f;
+  double sg = 0.0;                                 // PRB: this lane's share of the slope gradient
   float acc[ACC], sum[ACC];
   // A fragments (hi, lo) of two consecutive stages: stage kb's are written while the wgmmas of stage kb - 1, which read
   // the other set, are in flight
@@ -274,7 +294,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     int prev = 0;
     auto stage = [&](int kb, uint32_t (&h)[BK / 8][4], uint32_t (&l)[BK / 8][4]) {
       uint32_t wcur[2];
-      if (ACT && !STAT) {
+      if (PRO) {
         wcur[0] = wnext[0] >> (lane & 3); wcur[1] = wnext[1] >> (lane & 3);
         if (kb + 1 < num_kb) act_words(tile, kb + 1, wnext);
         else if (tile + (int)gridDim.x < num_tiles) act_words(tile + gridDim.x, 0, wnext);
@@ -292,6 +312,13 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             h[k][i] = act1(h[k][i], (i >> 1) ? t.z : t.x, (i >> 1) ? t.w : t.y, (wcur[i & 1] >> (8 * k + 4 * (i >> 1))) & 1u,
                            p.inv_keep);
         }
+      }
+      if (PRELU && !STAT) {
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)   // element i: row r0 + 8 (i % 2), column 8 k + lane % 4 + 4 (i / 2)
+            h[k][i] = prelu1(h[k][i], slope, (wcur[i & 1] >> (8 * k + 4 * (i >> 1))) & 1u, p.inv_keep);
       }
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k)
@@ -338,6 +365,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       const int col0 = n0 + c * 32;
       float4 xr[4], yr[4];
       if (STAT == 2) load_bn_chunk<ACT>(p, m0, col0, q, lane, xr, yr);
+      if (PRB) load_bn_chunk<true>(p, m0, col0, q, lane, xr, yr);   // Z only
       // accumulator fragment -> staging block, so that global stores are whole 128-byte row segments
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
@@ -368,6 +396,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           sh4 = __ldg(reinterpret_cast<const float4*>(p.act_shift + col0 + cq));
           load_bits_chunk(p, m0, col0, q, lane, wb);
         }
+        if (PRB) load_bits_chunk(p, m0, col0, q, lane, wb);
 #pragma unroll
         for (int it = 0; it < 4; ++it) {
           const int rr = it * 4 + sub;
@@ -405,11 +434,22 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
               s4.x += v.x; s4.y += v.y; s4.z += v.z; s4.w += v.w;
               q4.x = fmaf(v.x, (y.x - mu4.x) * is4.x, q4.x); q4.y = fmaf(v.y, (y.y - mu4.y) * is4.y, q4.y);
               q4.z = fmaf(v.z, (y.z - mu4.z) * is4.z, q4.z); q4.w = fmaf(v.w, (y.w - mu4.w) * is4.w, q4.w);
+            } else if (PRB) {
+              const float4 z = yr[it];
+              const uint32_t b = wb[it] >> cq;
+              const float gx = (b & 1u) ? v.x * p.inv_keep : 0.f, gy = (b & 2u) ? v.y * p.inv_keep : 0.f;
+              const float gz = (b & 4u) ? v.z * p.inv_keep : 0.f, gw = (b & 8u) ? v.w * p.inv_keep : 0.f;
+              if (!(z.x > 0.f)) sg += (double)(gx * z.x);
+              if (!(z.y > 0.f)) sg += (double)(gy * z.y);
+              if (!(z.z > 0.f)) sg += (double)(gz * z.z);
+              if (!(z.w > 0.f)) sg += (double)(gw * z.w);
+              v.x = z.x > 0.f ? gx : gx * slope; v.y = z.y > 0.f ? gy : gy * slope;
+              v.z = z.z > 0.f ? gz : gz * slope; v.w = z.w > 0.f ? gw : gw * slope;
             }
             *dst = v;
           }
         }
-        if (STAT) {
+        if (COLSTAT) {
           // 4 row sub-groups (lane >> 3) hold the same columns: fold them, lanes 0-7 add into the warp's accumulators
 #pragma unroll
           for (int d = 8; d <= 16; d <<= 1) {
@@ -455,11 +495,26 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
     }
   }
-  if (STAT) {
+  if (COLSTAT) {
     __syncwarp();
     float* out = p.stat_partial + (size_t)(blockIdx.x * CONSUMER_WARPS + q) * 2 * p.N;
     for (int i = lane; i < 2 * p.N; i += 32) out[i] = stat[i];
   }
+  if (PRB) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) sg += __shfl_xor_sync(0xffffffffu, sg, d);
+    if (lane == 0) p.slope_partial[blockIdx.x * CONSUMER_WARPS + q] = sg;
+  }
+}
+
+// slope_grad (+)= sum of the PRB partials in slot order (one warp, fixed order: bitwise repeatable)
+__global__ void __launch_bounds__(32) slope_grad_finalize_kernel(const double* __restrict__ part, int n, float* __restrict__ out,
+                                                                 int accumulate) {
+  double a = 0.0;
+  for (int i = threadIdx.x; i < n; i += 32) a += part[i];
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
+  if (threadIdx.x == 0) out[0] = accumulate ? out[0] + (float)a : (float)a;
 }
 
 // hi/lo split of a small matrix (weights), optionally transposed: out[c][r] when transpose.
@@ -489,7 +544,7 @@ static bool make_map(CUtensorMap* m, const float* base, int64_t rows, int64_t co
             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <class C, int STAT = 0, bool PEER = false, bool ACT = false>
+template <class C, int STAT = 0, bool PEER = false, bool ACT = false, bool PRELU = false>
 static int launch(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb, const Params& p,
                   cudaStream_t stream) {
   CUtensorMap tA, tBh, tBl, tX, tY;
@@ -504,14 +559,15 @@ static int launch(const float* A, int64_t lda, const float* B_hi, const float* B
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device and instantiation; idempotent if two threads race
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         C::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
     attr_set[dev] = true;
   }
   const int tiles = ((p.M + BM - 1) / BM) * ((p.N + C::BN - 1) / C::BN);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
-  gemm_tf32x3_kernel<C, STAT, PEER, ACT><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
+  gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
   return check_launch();
 }
 
@@ -534,10 +590,12 @@ static int g_bnbwd_variant = 0;   // A/B knob: 0 automatic, 1 force the TMA path
 extern "C" void b200gnn_gemm_set_bnbwd_variant(int v) { g_bnbwd_variant = v; }
 
 // st: the fused column statistics (stat_mode 1 / 2); act: the activation recomputed from Y (Params::act_*, inv_keep) — of the
-// A operand without st, of the BatchNorm-backward mask with stat_mode 2.
+// A operand without st, of the BatchNorm-backward mask with stat_mode 2; prelu: the PReLU/dropout prologue (stat_mode 0) or
+// backward epilogue (stat_mode 4) of Params::act_slope / act_bits.
 static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb, float* C, int64_t ldc,
                          int64_t M, int64_t N, int64_t K, const float* bias, int accumulate, void* stream,
-                         const gemm::Params* st = nullptr, const gemm::Params* act = nullptr) {
+                         const gemm::Params* st = nullptr, const gemm::Params* act = nullptr,
+                         const gemm::Params* prelu = nullptr) {
   if (!A || !B_hi || !B_lo || !C || M <= 0 || N <= 0 || K <= 0 || lda < K || ldb < K || ldc < N ||
       M >= INT32_MAX || N >= INT32_MAX || K >= INT32_MAX)
     return B200GNN_ERR_BAD_ARG;
@@ -552,6 +610,19 @@ static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const f
       return B200GNN_ERR_BAD_ARG;
     p.act_scale = act->act_scale; p.act_shift = act->act_shift; p.act_bits = act->act_bits; p.act_words = act->act_words;
     p.inv_keep = act->inv_keep;
+  }
+  if (prelu) {
+    if (!prelu->act_slope || !prelu->act_bits) return B200GNN_ERR_BAD_ARG;
+    p.act_slope = prelu->act_slope; p.act_bits = prelu->act_bits; p.act_words = prelu->act_words; p.inv_keep = prelu->inv_keep;
+    if (prelu->stat_mode == 0) {
+      if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>, 0, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+      return gemm::launch<gemm::Cfg<128, 4>, 0, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    }
+    // backward epilogue: whole 32-column chunks through the vectorised epilogue only
+    if (N % 32 || ldc % 4 || !aligned_to(C, 16) || !prelu->bn_y || !aligned_to(prelu->bn_y, 16) || !prelu->slope_partial)
+      return B200GNN_ERR_UNSUPPORTED;
+    p.stat_mode = 4; p.bn_y = prelu->bn_y; p.slope_partial = prelu->slope_partial;
+    return gemm::launch<gemm::Cfg<128, 4>, 4>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
   }
   if (act && !st) {
     // (scale, shift) of all K columns in the statistics block of shared memory
@@ -645,6 +716,41 @@ extern "C" int b200gnn_gemm_tf32x3_act_f32(const float* Y, int64_t lda, const fl
   act.act_scale = scale; act.act_shift = shift; act.act_bits = bits; act.act_words = (int32_t)((K + 31) / 32);
   act.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
   return gemm_dispatch(Y, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, bias, 0, stream, nullptr, &act);
+}
+
+// C = dropout(prelu(Z)) · B^T (+ bias) with the activation formed in the GEMM's registers from Z, the slope (device scalar)
+// and the packed keep bits (uint32 [M][ceil(K / 32)]): bit for bit the GEMM of the activation b200gnn_prelu_bits_f32
+// materialises.  Any K (no per-column table).
+extern "C" int b200gnn_gemm_tf32x3_prelu_f32(const float* Z, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                             float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                             const float* slope, const uint32_t* bits, float p_drop, void* stream) {
+  if (p_drop < 0.f || p_drop >= 1.f) return B200GNN_ERR_BAD_ARG;
+  gemm::Params pr{};
+  pr.stat_mode = 0; pr.act_slope = slope; pr.act_bits = bits; pr.act_words = (int32_t)((K + 31) / 32);
+  pr.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  return gemm_dispatch(Z, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, bias, 0, stream, nullptr, nullptr, &pr);
+}
+
+// The input-gradient GEMM behind x = dropout(prelu(Z)): dA = A · B^T (+ C when accumulate); what is STORED to C is
+// dZ = (bit ? dA / (1-p) : 0) * (Z > 0 ? 1 : slope), and slope_grad (+)= sum of (bit ? dA / (1-p) : 0) * Z over Z <= 0,
+// reduced in fp64 per consumer warp (partial: double[slots], slots >= b200gnn_gemm_stat_slots(M, N)) and then in slot order.
+// Z: [M, ldc] like C; bits: uint32 [M][N / 32]; N a multiple of 32.
+extern "C" int b200gnn_gemm_tf32x3_prelu_bwd_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                                 float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
+                                                 const float* Z, const uint32_t* bits, const float* slope, float p_drop,
+                                                 float* slope_grad, int slope_accumulate, double* partial, int64_t slots,
+                                                 void* stream) {
+  if (!Z || !slope_grad || !partial || p_drop < 0.f || p_drop >= 1.f || M <= 0 || N <= 0) return B200GNN_ERR_BAD_ARG;
+  const int64_t used = b200gnn_gemm_stat_slots(M, N);
+  if (slots < used) return B200GNN_ERR_BAD_ARG;
+  gemm::Params pr{};
+  pr.stat_mode = 4; pr.act_slope = slope; pr.act_bits = bits; pr.act_words = (int32_t)((N + 31) / 32);
+  pr.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  pr.bn_y = Z; pr.slope_partial = partial;
+  int rc = gemm_dispatch(A, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, nullptr, accumulate, stream, nullptr, nullptr, &pr);
+  if (rc) return rc;
+  gemm::slope_grad_finalize_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(partial, (int)used, slope_grad, slope_accumulate ? 1 : 0);
+  return check_launch();
 }
 
 extern "C" int b200gnn_gemm_tf32x3_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,

@@ -51,9 +51,14 @@ struct Params {
   const uint32_t* act_bits;
   int32_t act_words;
   float inv_keep;
+  // PRELU: X is the pre-activation Z of a SIGN FeedForwardNet layer and the operand is dropout(prelu(Z)), recomputed with the
+  // slope (device scalar) exactly as gemm_tf32x3.cu's PRELU prologue does; the keep bits have a row pitch of act_ld words
+  // (column blocks of a wider Z: act_words = ceil(Kin / 32) bound the block)
+  const float* act_slope;
+  int32_t act_ld;
 };
 
-template <bool ACT>
+template <bool ACT, bool PRELU = false>
 __global__ void __launch_bounds__(THREADS, 1)
 wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG, const Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -105,10 +110,13 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   const int pair = cw * 32 + (warp & 3) * 8 + (lane >> 2);
   const int c0 = mt * TM + cw * 64 + (warp & 3) * 16 + (lane >> 2);
   uint32_t wnext = 0u;
+  const int bits_ld = PRELU ? p.act_ld : p.act_words;
   auto act_word = [&](int kb) {
     const int node = kb * BKN + lane;
-    return node < p.Nn && (c0 >> 5) < p.act_words ? __ldg(p.act_bits + (size_t)node * p.act_words + (c0 >> 5)) : 0u;
+    return node < p.Nn && (c0 >> 5) < p.act_words ? __ldg(p.act_bits + (size_t)node * bits_ld + (c0 >> 5)) : 0u;
   };
+  const float slope = PRELU ? __ldg(p.act_slope) : 0.f;
+  if (PRELU && kb0 < kb1) wnext = act_word(kb0);
   if (ACT) {
     if (ct < TM / 2) {
       const int c = mt * TM + (ct >> 3) * 16 + (ct & 7);   // pair ct: columns c, c + 8
@@ -127,7 +135,7 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   int s = 0; uint32_t ph = 0;
   auto block = [&](int i, uint32_t (&h)[BKN / 8][4], uint32_t (&l)[BKN / 8][4]) {
     uint32_t wcur = 0u;
-    if (ACT) {
+    if (ACT || PRELU) {
       wcur = wnext;
       if (kb0 + i + 1 < kb1) wnext = act_word(kb0 + i + 1);
     }
@@ -138,6 +146,7 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
       ss = act_ss[pair];
       asm volatile("" : "+r"(l4));             // shuffle source lanes formed per block, not held in 8 registers
     }
+    if (PRELU) asm volatile("" : "+r"(l4));
     const uint32_t sraw = smem_u32(smem + s * RAW_BYTES);
     const float* rg = reinterpret_cast<const float*>(smem + s * RAW_BYTES + BKN * TM * 4);   // [32 nodes][128]
     uint8_t* T = tbuf + (i & 1) * T_BYTES;
@@ -164,6 +173,12 @@ wgrad_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
         if (ACT) {
           const uint32_t w = __shfl_sync(0xffffffffu, wcur, 8 * k + l4 + 4 * (j >> 1));
           const float y = fmaxf(fmaf(__uint_as_float(v), (j & 1) ? ss.z : ss.x, (j & 1) ? ss.w : ss.y), 0.f) * p.inv_keep;
+          v = (w >> ((c0 & 31) + 8 * (j & 1))) & 1u ? __float_as_uint(y) : 0u;
+        }
+        if (PRELU) {                             // the same operations as b200gnn_prelu_bits_f32
+          const uint32_t w = __shfl_sync(0xffffffffu, wcur, 8 * k + l4 + 4 * (j >> 1));
+          const float z = __uint_as_float(v);
+          const float y = (z > 0.f ? z : slope * z) * p.inv_keep;
           v = (w >> ((c0 & 31) + 8 * (j & 1))) & 1u ? __float_as_uint(y) : 0u;
         }
         split1(v, h[k][j], l[k][j]);
@@ -276,7 +291,7 @@ extern "C" int64_t b200gnn_wgrad_workspace_floats(int64_t Kin, int64_t Nout) {
   return wgrad::range_cap(Kin, Nout) * wgrad::pad_k(Kin) * wgrad::pad_n(Nout);
 }
 
-template <bool ACT>
+template <bool ACT, bool PRELU = false>
 static int wgrad_launch(const float* X, int64_t ldx, const float* G, int64_t ldg, float* dW, int64_t Nn, int64_t Kin, int64_t Nout,
                         float* workspace, const wgrad::Params& act, void* stream) {
   if (!X || !G || !dW || !workspace || Nn <= 0 || Kin <= 0 || Nout <= 0 || ldx < Kin || ldg < Nout || Nn >= INT32_MAX)
@@ -293,7 +308,7 @@ static int wgrad_launch(const float* X, int64_t ldx, const float* G, int64_t ldg
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad::wgrad_tf32x3_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(wgrad::wgrad_tf32x3_kernel<ACT, PRELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          wgrad::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
     attr_set[dev] = true;
@@ -314,7 +329,7 @@ static int wgrad_launch(const float* X, int64_t ldx, const float* G, int64_t ldg
   if (ranges < 1) ranges = 1;
   p.n_ranges = ranges;
   int rc;
-  wgrad::wgrad_tf32x3_kernel<ACT><<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
+  wgrad::wgrad_tf32x3_kernel<ACT, PRELU><<<tiles * ranges, wgrad::THREADS, wgrad::SMEM_BYTES, st>>>(tX, tG, p);
   if ((rc = check_launch())) return rc;
   const int64_t n_vec = (int64_t)p.Kpad * p.Npad / 4;
   wgrad::wgrad_reduce_kernel<<<(int)((n_vec + wgrad::RED_VECS - 1) / wgrad::RED_VECS), wgrad::RED_VECS * wgrad::RED_GROUPS, 0, st>>>(
@@ -337,4 +352,20 @@ extern "C" int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, co
   act.act_scale = scale; act.act_shift = shift; act.act_bits = bits; act.act_words = (int32_t)((Kin + 31) / 32);
   act.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
   return wgrad_launch<true>(Y, ldx, G, ldg, dW, Nn, Kin, Nout, workspace, act, stream);
+}
+
+// dW = dropout(prelu(Z))^T · G with the activation recomputed from Z, the slope (device scalar) and the packed keep bits
+// (uint32, row pitch ldbits words, bit c of the block's column c): bit for bit the weight gradient of the activation
+// b200gnn_prelu_bits_f32 materialises.  Kin <= 2048 as above; a wider Z (SIGN's [B, hops * hidden] concatenation) is
+// passed as column blocks: Z + c0, bits + c0 / 32, dW + c0 * Nout for c0 a multiple of 32.
+extern "C" int b200gnn_gemm_wgrad_tf32x3_prelu_f32(const float* Z, int64_t ldz, const float* G, int64_t ldg, float* dW,
+                                                   int64_t Nn, int64_t Kin, int64_t Nout, const float* slope,
+                                                   const uint32_t* bits, int64_t ldbits, float p_drop, float* workspace,
+                                                   void* stream) {
+  if (!slope || !bits || ldbits < (Kin + 31) / 32 || ldbits >= INT32_MAX || p_drop < 0.f || p_drop >= 1.f)
+    return B200GNN_ERR_BAD_ARG;
+  wgrad::Params act{};
+  act.act_slope = slope; act.act_bits = bits; act.act_words = (int32_t)((Kin + 31) / 32); act.act_ld = (int32_t)ldbits;
+  act.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  return wgrad_launch<false, true>(Z, ldz, G, ldg, dW, Nn, Kin, Nout, workspace, act, stream);
 }

@@ -24,4 +24,25 @@ __host__ __device__ __forceinline__ uint4 philox4x32(uint64_t seed, uint64_t off
 // uniform in [0,1) with 24 bits (exactly representable in fp32)
 __host__ __device__ __forceinline__ float u32_to_unit(uint32_t x) { return (float)(x >> 8) * (1.0f / 16777216.0f); }
 
+// The dropout keep decisions of four consecutive elements (one float4):
+//   keep16: p * 65536 integral (dropout_p16), two 16-bit uniforms of a Philox word each, keep iff u16 >= p * 65536 — exact;
+//   keep24: otherwise, four 24-bit uniforms of one Philox block, keep iff u >= p.
+__device__ __forceinline__ uchar4 keep16(uint32_t a, uint32_t b, uint32_t thr) {
+  uchar4 m;
+  m.x = (a & 0xffffu) >= thr; m.y = (a >> 16) >= thr; m.z = (b & 0xffffu) >= thr; m.w = (b >> 16) >= thr;
+  return m;
+}
+__device__ __forceinline__ uchar4 keep24(const uint4& r, float p) {
+  uchar4 m;
+  m.x = u32_to_unit(r.x) >= p; m.y = u32_to_unit(r.y) >= p; m.z = u32_to_unit(r.z) >= p; m.w = u32_to_unit(r.w) >= p;
+  return m;
+}
+
+// p * 65536 integral (and p > 0): the 16-bit decision path is exact
+static inline bool dropout_p16(float p, uint32_t& thr16) {
+  const double t = (double)p * 65536.0;
+  thr16 = (uint32_t)t;
+  return p > 0.f && t == (double)thr16;
+}
+
 }  // namespace b200gnn

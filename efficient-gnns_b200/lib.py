@@ -91,6 +91,17 @@ SIGNATURES = {
     "b200gnn_gemm_wgrad_tf32x3_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gemm_wgrad_tf32x3_act_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _f32p, _ptr, _f32,
                                                  _f32p, _ptr]),
+    "b200gnn_gemm_tf32x3_prelu_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p,
+                                             _f32p, _ptr, _f32, _ptr]),
+    "b200gnn_gemm_tf32x3_prelu_bwd_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _int,
+                                                 _f32p, _ptr, _f32p, _f32, _f32p, _int, _ptr, _i64, _ptr]),
+    "b200gnn_gemm_wgrad_tf32x3_prelu_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _ptr, _i64, _f32,
+                                                   _f32p, _ptr]),
+    "b200gnn_prelu_bits_f32": (_int, [_f32p, _i64, _ptr, _i64, _f32p, _f32, _f32p, _i64, _i64, _i64, _ptr]),
+    "b200gnn_sign_gather_f32": (_int, [_ptr, _i32, _i64, _i64, _ptr, _i64, _f32, _u64, _u64, _i32p, _u64, _f32p, _ptr, _ptr,
+                                       _f32p, _i64, _i64, _f32p, _ptr]),
+    "b200gnn_col_sum_ld_slots": (_i64, [_i64]),
+    "b200gnn_col_sum_ld_f32": (_int, [_f32p, _i64, _i64, _i64, _f32p, _f32p, _i64, _ptr]),
     "b200gnn_row_normalize_fwd_f32": (_int, [_f32p, _i64, _i64, _f32, _f32, _f32p, _f32p, _ptr]),
     "b200gnn_row_normalize_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _f32, _f32p, _int, _ptr]),
     "b200gnn_reduce_slots": (_i64, [_i64]),

@@ -564,3 +564,163 @@ def embedding_adam(d_out: torch.Tensor, node_type: torch.Tensor, local_idx: torc
         _f32(table, "table"), _f32(exp_avg, "exp_avg"), _f32(exp_avg_sq, "exp_avg_sq"), rows, F_,
         lib.dptr(head, torch.int32, "head"), lr, betas[0], betas[1], eps, lib.dptr(step, torch.int32, "step"), lib.stream_ptr()),
         "embedding_adam_f32")
+
+
+# ----------------------------------------------------------------------------- SIGN (PReLU FeedForwardNet layers)
+def _rows(t: torch.Tensor, name: str):
+    """(device pointer, row pitch) of an fp32 CUDA matrix whose rows are contiguous (column blocks of a wider matrix pass)."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+        raise lib.B200GnnError(f"{name}: expected a CUDA float32 matrix with contiguous rows")
+    return t.data_ptr(), t.stride(0)
+
+
+def _bits_rows(bits: torch.Tensor, n: int, K: int):
+    """(pointer, row pitch in words) of int32 keep bits covering rows [0, n) and columns [0, K)."""
+    if bits.dtype != torch.int32 or not bits.is_cuda or bits.dim() != 2 or bits.stride(1) != 1 or bits.shape[0] != n \
+            or bits.shape[1] < (K + 31) // 32:
+        raise lib.B200GnnError(f"keep bits: expected CUDA int32 [{n}, >= {(K + 31) // 32}] with contiguous rows")
+    return bits.data_ptr(), bits.stride(0)
+
+
+def prelu_bits(z: torch.Tensor, bits: torch.Tensor, slope: torch.Tensor, p: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dropout(prelu(z)) with the keep decisions of ``dropout_bits`` and the slope scalar (device): what the PReLU GEMM
+    prologues form in registers, materialised."""
+    n, K = z.shape
+    if out is None:
+        out = torch.empty(n, K, dtype=torch.float32, device=z.device)
+    zp, ldz = _rows(z, "z")
+    op, ldo = _rows(out, "out")
+    bp, ldb = _bits_rows(bits, n, K)
+    lib.check(lib.load().b200gnn_prelu_bits_f32(zp, ldz, bp, ldb, _f32(slope, "slope"), float(p), op, ldo, n, K, lib.stream_ptr()),
+              "prelu_bits_f32")
+    return out
+
+
+def gemm_tf32x3_prelu(z: torch.Tensor, slope: torch.Tensor, bits: torch.Tensor, p: float, b_hi: torch.Tensor, b_lo: torch.Tensor,
+                      bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = dropout(prelu(z)) @ b^T (+bias), the activation formed in the GEMM's registers: bit for bit gemm_tf32x3 of
+    ``prelu_bits``.  ``out`` may be a column block of a wider matrix (row pitch taken from its stride)."""
+    M, K = z.shape
+    N = b_hi.shape[0]
+    assert b_hi.shape == b_lo.shape and b_hi.shape[1] == K
+    if out is None:
+        out = torch.empty(M, N, dtype=torch.float32, device=z.device)
+    zp, lda = _rows(z, "z")
+    op, ldc = _rows(out, "out")
+    if bits.shape[1] != (K + 31) // 32:
+        raise lib.B200GnnError("gemm_tf32x3_prelu: keep bits must be [M, ceil(K/32)]")
+    lib.check(lib.load().b200gnn_gemm_tf32x3_prelu_f32(zp, lda, _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"), b_hi.stride(0), op, ldc, M, N, K,
+                                                       _f32(bias, "bias"), _f32(slope, "slope"), _bits(bits, M, K), float(p),
+                                                       lib.stream_ptr()), "gemm_tf32x3_prelu_f32")
+    return out
+
+
+def gemm_tf32x3_prelu_bwd(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, out: torch.Tensor, z: torch.Tensor,
+                          bits: torch.Tensor, slope: torch.Tensor, p: float, slope_grad: torch.Tensor, partial: torch.Tensor,
+                          accumulate: bool = False, slope_accumulate: bool = False) -> torch.Tensor:
+    """Input-gradient GEMM behind x = dropout(prelu(z)): d_x = a @ b^T (+ out if accumulate); STORES
+    dz = d_x * keep / (1-p) * (z > 0 ? 1 : slope) to ``out`` and writes (or adds, slope_accumulate) the slope gradient to
+    slope_grad[0].  ``a`` may be a column block (row pitch from its stride); partial: float64 [gemm_stat_slots(M, N)]."""
+    M, K = a.shape
+    N = b_hi.shape[0]
+    assert out.shape == z.shape == (M, N) and out.stride(0) == z.stride(0)
+    if partial.dtype != torch.float64 or not partial.is_cuda or partial.numel() < gemm_stat_slots(M, N):
+        raise lib.B200GnnError("gemm_tf32x3_prelu_bwd: partial must be CUDA float64 [>= gemm_stat_slots(M, N)]")
+    ap, lda = _rows(a, "a")
+    op, ldc = _rows(out, "out")
+    lib.check(lib.load().b200gnn_gemm_tf32x3_prelu_bwd_f32(ap, lda, _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"), b_hi.stride(0), op, ldc,
+                                                           M, N, K, int(accumulate), _rows(z, "z")[0], _bits(bits, M, N),
+                                                           _f32(slope, "slope"), float(p), slope_grad.data_ptr(),
+                                                           int(slope_accumulate), partial.data_ptr(), partial.numel(),
+                                                           lib.stream_ptr()), "gemm_tf32x3_prelu_bwd_f32")
+    return out
+
+
+WGRAD_PRELU_BLOCK = 512   # column block of a Z wider than the kernel's 2048-column tiling
+
+
+def gemm_wgrad_tf32x3_prelu(z: torch.Tensor, slope: torch.Tensor, bits: torch.Tensor, p: float, g: torch.Tensor,
+                            out: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[Kin, Nout] = dropout(prelu(z))^T @ g, the activation formed in registers (bit for bit gemm_wgrad_tf32x3 of
+    ``prelu_bits``).  Kin > 2048 runs as 512-column blocks of z.  z and g may be column blocks (row pitches from strides)."""
+    nn_, k_in = z.shape
+    n_out = g.shape[1]
+    assert g.shape[0] == nn_
+    if k_in % 4 or n_out % 4:
+        raise lib.B200GnnError(f"gemm_wgrad_tf32x3_prelu: Kin={k_in}, Nout={n_out} must be multiples of 4")
+    L = lib.load()
+    if out is None:
+        out = torch.empty(k_in, n_out, dtype=torch.float32, device=z.device)
+    blk = k_in if k_in <= 2048 else WGRAD_PRELU_BLOCK
+    if workspace is None:
+        workspace = torch.empty(wgrad_workspace_floats(blk, n_out), dtype=torch.float32, device=z.device)
+    bp, ldb = _bits_rows(bits, nn_, k_in)
+    gp, ldg = _rows(g, "g")
+    assert out.is_contiguous()
+    for c0 in range(0, k_in, blk):
+        kb = min(blk, k_in - c0)
+        zb, ldz = _rows(z[:, c0:c0 + kb], "z")
+        lib.check(L.b200gnn_gemm_wgrad_tf32x3_prelu_f32(zb, ldz, gp, ldg, out[c0:c0 + kb].data_ptr(), nn_, kb, n_out,
+                                                        _f32(slope, "slope"), bp + 4 * (c0 // 32), ldb, float(p),
+                                                        _f32(workspace, "workspace"), lib.stream_ptr()),
+                  "gemm_wgrad_tf32x3_prelu_f32")
+    return out
+
+
+def gemm_wgrad_tf32x3_rows(x: torch.Tensor, g: torch.Tensor, out: torch.Tensor, workspace: torch.Tensor) -> torch.Tensor:
+    """gemm_wgrad_tf32x3 (any tiling it accepts) on operands that may be column blocks of wider matrices."""
+    nn_, k_in = x.shape
+    xp, ldx = _rows(x, "x")
+    gp, ldg = _rows(g, "g")
+    lib.check(lib.load().b200gnn_gemm_wgrad_tf32x3_f32(xp, ldx, gp, ldg, _f32(out, "out"), nn_, k_in, g.shape[1],
+                                                       _f32(workspace, "workspace"), lib.stream_ptr()), "gemm_wgrad_tf32x3_f32")
+    return out
+
+
+def gemm_tf32x3_rows(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, out: torch.Tensor,
+                     bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemm_tf32x3 with ``a`` / ``out`` possibly column blocks of wider matrices (row pitches from strides)."""
+    M, K = a.shape
+    N = b_hi.shape[0]
+    ap, lda = _rows(a, "a")
+    op, ldc = _rows(out, "out")
+    lib.check(lib.load().b200gnn_gemm_tf32x3_f32(ap, lda, _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"), b_hi.stride(0), op, ldc, M, N, K,
+                                                 _f32(bias, "bias"), lib.stream_ptr()), "gemm_tf32x3_f32")
+    return out
+
+
+def col_sum_ld(y: torch.Tensor, out: torch.Tensor, partial: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[K] = column sums of y [n, K] (rows contiguous, any pitch), fixed summation order."""
+    n, K = y.shape
+    L = lib.load()
+    slots = int(L.b200gnn_col_sum_ld_slots(n))
+    if partial is None:
+        partial = torch.empty(slots * K, dtype=torch.float32, device=y.device)
+    yp, ldy = _rows(y, "y")
+    lib.check(L.b200gnn_col_sum_ld_f32(yp, ldy, n, K, _f32(out, "out"), partial.data_ptr(), partial.numel() // K, lib.stream_ptr()),
+              "col_sum_ld_f32")
+    return out
+
+
+def sign_gather(feats, idx: torch.Tensor, p: float, seed: int, offset: int, out: torch.Tensor,
+                step_dev: Optional[torch.Tensor] = None, step_mul: int = 0, labels: Optional[torch.Tensor] = None,
+                labels_out: Optional[torch.Tensor] = None, teacher: Optional[torch.Tensor] = None,
+                teacher_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[h, i] = input_dropout(feats[h][idx[i]]) for every hop (hop h: the mask of dropout_mask(B, F, p, seed,
+    offset + h + step * step_mul)), plus the batch's label and teacher-logit rows."""
+    H = len(feats)
+    B = idx.numel()
+    n, F_ = feats[0].shape
+    for f in feats:
+        if f.shape != (n, F_):
+            raise lib.B200GnnError("sign_gather: every hop feature matrix must have the same shape")
+        _f32(f, "feats")
+    assert out.shape == (H, B, F_)
+    C = teacher.shape[1] if teacher is not None else 0
+    lib.check(lib.load().b200gnn_sign_gather_f32(
+        _host_ptr_array([f.data_ptr() for f in feats]), H, n, F_, lib.dptr(idx, torch.int64, "idx"), B, float(p), int(seed),
+        int(offset), lib.dptr(step_dev, torch.int32, "step_dev"), int(step_mul), _f32(out, "out"),
+        lib.dptr(labels, torch.int64, "labels"), lib.dptr(labels_out, torch.int64, "labels_out"),
+        _f32(teacher, "teacher"), teacher.stride(0) if teacher is not None else 0, C, _f32(teacher_out, "teacher_out"),
+        lib.stream_ptr()), "sign_gather_f32")
+    return out

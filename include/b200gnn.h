@@ -349,6 +349,50 @@ int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, const float* 
                                       const uint32_t* bits, float p_drop, float* workspace, void* stream);
 
 /* ------------------------------------------------------------------ *
+ * SIGN student (arxiv_dgl/sign.py:105-157): FeedForwardNet layers Linear -> PReLU (one learnable slope, a device scalar)
+ * -> dropout, with the activation x = dropout(prelu(Z)) never materialised in training.  bits: packed keep decisions of
+ * b200gnn_dropout_bits_u32 (bit c % 32 of word c / 32 of a row).
+ *   _gemm_tf32x3_prelu_f32      : C = x · B^T (+ bias), x formed from Z in the GEMM's registers (bits uint32 [M][ceil(K/32)]),
+ *                                 bit for bit the product of the activation b200gnn_prelu_bits_f32 materialises.  Any K.
+ *   _gemm_tf32x3_prelu_bwd_f32  : the input-gradient GEMM behind x: dA = A · B^T (+ C if accumulate); what is STORED to C is
+ *                                 dZ = (bit ? dA/(1-p) : 0) * (Z > 0 ? 1 : slope) (Z: [M, ldc] like C, bits [M][N/32], N a
+ *                                 multiple of 32); slope_grad = (slope_accumulate ? slope_grad : 0) + sum over Z <= 0 of
+ *                                 (bit ? dA/(1-p) : 0) * Z, reduced in fp64 per consumer warp into partial (double[slots],
+ *                                 slots >= b200gnn_gemm_stat_slots(M, N)) and then in slot order: no atomics, repeatable.
+ *   _gemm_wgrad_tf32x3_prelu_f32: dW = x^T · G as b200gnn_gemm_wgrad_tf32x3_f32 (Kin <= 2048), bits with a row pitch of ldbits
+ *                                 words so that a wider Z runs as column blocks (Z + c0, bits + c0/32, dW + c0*Nout).
+ *   _prelu_bits_f32             : out = x materialised (row pitches ldz / ldbits / ldo).
+ *   _sign_gather_f32            : out[h][i] = dropout_p(feats[h][idx[i]]) for the n_hops HOST-array device pointers feats[h]
+ *                                 ([n_nodes, F] each, F % 4 == 0); hop h draws the mask b200gnn_dropout_mask_u8(B, F, p, seed,
+ *                                 offset + h + *step_dev * step_mul) takes.  Also labels_out[i] = labels[idx[i]] and
+ *                                 teacher_out[i] = teacher[idx[i]] ([B, C], teacher pitch ldt) when given.  Indices outside
+ *                                 [0, n_nodes) gather zero rows.
+ *   _col_sum_ld_f32             : out[K] = column sums of Y [n_rows, K] with row pitch ldy (partial: float[slots * K], slots >=
+ *                                 b200gnn_col_sum_ld_slots(n_rows)); fixed summation order.
+ * ------------------------------------------------------------------ */
+int b200gnn_gemm_tf32x3_prelu_f32(const float* Z, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                  float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                  const float* slope, const uint32_t* bits, float p_drop, void* stream);
+int b200gnn_gemm_tf32x3_prelu_bwd_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                      float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
+                                      const float* Z, const uint32_t* bits, const float* slope, float p_drop,
+                                      float* slope_grad, int slope_accumulate, double* partial, int64_t slots,
+                                      void* stream);
+int b200gnn_gemm_wgrad_tf32x3_prelu_f32(const float* Z, int64_t ldz, const float* G, int64_t ldg, float* dW,
+                                        int64_t Nn, int64_t Kin, int64_t Nout, const float* slope,
+                                        const uint32_t* bits, int64_t ldbits, float p_drop, float* workspace,
+                                        void* stream);
+int b200gnn_prelu_bits_f32(const float* Z, int64_t ldz, const uint32_t* bits, int64_t ldbits, const float* slope, float p,
+                           float* out, int64_t ldo, int64_t n_rows, int64_t K, void* stream);
+int b200gnn_sign_gather_f32(const float* const* feats, int32_t n_hops, int64_t n_nodes, int64_t F, const int64_t* idx,
+                            int64_t B, float p, uint64_t seed, uint64_t offset, const int32_t* step_dev,
+                            uint64_t step_mul, float* out, const int64_t* labels, int64_t* labels_out,
+                            const float* teacher, int64_t ldt, int64_t C, float* teacher_out, void* stream);
+int64_t b200gnn_col_sum_ld_slots(int64_t n_rows);
+int b200gnn_col_sum_ld_f32(const float* Y, int64_t ldy, int64_t n_rows, int64_t K, float* out, float* partial,
+                           int64_t slots, void* stream);
+
+/* ------------------------------------------------------------------ *
  * Feature-distillation criteria (arxiv_pyg/criterion.py): row / pair passes.
  * The S x S contractions (G-CRD logits, GSP Gram matrices) run on
  * b200gnn_gemm_tf32x3_f32; these kernels are the passes around them.
