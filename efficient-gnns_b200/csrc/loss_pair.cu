@@ -142,16 +142,20 @@ __global__ void __launch_bounds__(256) nce_rows_kernel(float* __restrict__ Z, in
 }
 
 // ---------------------------------------------------------------- tiled transpose  out[c][r] = in[r][c]
+// gridDim.y is capped at 65,535 row tiles (2,097,120 rows), so each CTA walks its row tiles with a grid stride.
 __global__ void __launch_bounds__(256) transpose_kernel(const float* __restrict__ in, int64_t rows, int64_t cols,
                                                         float* __restrict__ out) {
   __shared__ float tile[32][33];
-  const int64_t c0 = (int64_t)blockIdx.x * 32, r0 = (int64_t)blockIdx.y * 32;
+  const int64_t c0 = (int64_t)blockIdx.x * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
-  for (int i = ty; i < 32; i += 8)
-    if (r0 + i < rows && c0 + tx < cols) tile[i][tx] = in[(size_t)(r0 + i) * cols + c0 + tx];
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8)
-    if (c0 + i < cols && r0 + tx < rows) out[(size_t)(c0 + i) * rows + r0 + tx] = tile[tx][i];
+  for (int64_t r0 = (int64_t)blockIdx.y * 32; r0 < rows; r0 += (int64_t)gridDim.y * 32) {
+    for (int i = ty; i < 32; i += 8)
+      if (r0 + i < rows && c0 + tx < cols) tile[i][tx] = in[(size_t)(r0 + i) * cols + c0 + tx];
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8)
+      if (c0 + i < cols && r0 + tx < rows) out[(size_t)(c0 + i) * rows + r0 + tx] = tile[tx][i];
+    __syncthreads();   // the tile is refilled by the next row tile
+  }
 }
 
 // ---------------------------------------------------------------- GSP: pairwise-similarity MSE
@@ -335,7 +339,8 @@ extern "C" int b200gnn_nce_finish_f32(const float* partial, int64_t S, float* lo
 
 extern "C" int b200gnn_transpose_f32(const float* in, int64_t rows, int64_t cols, float* out, void* stream) {
   if (!in || !out || rows <= 0 || cols <= 0) return B200GNN_ERR_BAD_ARG;
-  dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
+  const int64_t row_tiles = (rows + 31) / 32;
+  dim3 grid((unsigned)((cols + 31) / 32), (unsigned)(row_tiles < 65535 ? row_tiles : 65535));
   transpose_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, rows, cols, out);
   return check_launch();
 }
