@@ -258,6 +258,24 @@ __global__ void __launch_bounds__(256) dropout_mask_kernel(uint8_t* __restrict__
   }
 }
 
+// dropout_mask_kernel with the effective offset read on the device (offset + *step_dev * step_mul): a captured CUDA graph
+// draws a fresh mask on every replay (the GAT step's edge drop).
+__global__ void __launch_bounds__(256) dropout_mask_step_kernel(uint8_t* __restrict__ mask, int64_t n_vec, float p, int p16,
+                                                                uint32_t thr16, uint64_t seed, uint64_t offset,
+                                                                const int32_t* __restrict__ step_dev, uint64_t step_mul) {
+  const uint64_t off = offset + (uint64_t)(*step_dev) * step_mul;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (int64_t)gridDim.x * blockDim.x) {
+    uchar4 m;
+    if (p16) {
+      const uint4 r = philox4x32(seed, off, (uint64_t)i >> 1);
+      m = keep16((i & 1) ? r.z : r.x, (i & 1) ? r.w : r.y, thr16);
+    } else {
+      m = keep24(philox4x32(seed, off, (uint64_t)i), p);
+    }
+    reinterpret_cast<uchar4*>(mask)[i] = m;
+  }
+}
+
 // The same keep decisions packed one bit per element for n_layers hidden layers at once: layer l (offset + l, plus
 // step_dev * step_mul) fills bits[l][row][w], bit b = column 32 w + b (zero past K).  One thread per word; consecutive float4s
 // of a word share their Philox block in the P16 path.  The GEMMs recompute the activation from Y and these bits
@@ -571,6 +589,18 @@ extern "C" int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K,
   uint32_t thr16 = 0;
   const int p16 = dropout_p16(p, thr16) ? 1 : 0;
   dropout_mask_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(mask, n_vec, p, p16, thr16, seed, offset);
+  return check_launch();
+}
+
+extern "C" int b200gnn_dropout_mask_step_u8(uint8_t* mask, int64_t n_rows, int64_t K, float p, uint64_t seed, uint64_t offset,
+                                            const int32_t* step_dev, uint64_t step_mul, void* stream) {
+  if (!rows_ok(n_rows, K) || !mask || !step_dev || p < 0.f || p >= 1.f) return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  const int64_t n_vec = n_rows * (K / 4);
+  uint32_t thr16 = 0;
+  const int p16 = dropout_p16(p, thr16) ? 1 : 0;
+  dropout_mask_step_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(mask, n_vec, p, p16, thr16, seed, offset,
+                                                                                      step_dev, step_mul);
   return check_launch();
 }
 

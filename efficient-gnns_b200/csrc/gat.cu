@@ -191,9 +191,10 @@ __device__ __forceinline__ void hub_segment(const int32_t* rowptr, const int32_t
 
 // lane handles vectors v = lane + 32*j (j < NJ) of width W; head of vector v = (v*W)/D.  The group's warps take
 // groups of U consecutive edges: warp `first` of `stride` warps starts at beg + first*U.
-template <typename V, int NJ, int U>
+// SS: the coefficient of edge k is a[k,h] * src_scale[col[k]] (the fused layer's out_deg^-1/2, or 1 when the vector is absent).
+template <typename V, int NJ, int U, bool SS = false>
 __device__ __forceinline__ void agg_edges(const GatAgg& p, int beg, int end, int first, int stride, int lane, int nvec,
-                                          const int (&head)[NJ], V (&acc)[NJ]) {
+                                          const int (&head)[NJ], V (&acc)[NJ], const float* src_scale = nullptr) {
   constexpr int W = VecTraits<V>::W;
   const V* F = reinterpret_cast<const V*>(p.ft);
   const size_t ldv = (size_t)(p.ldf / W);
@@ -204,11 +205,14 @@ __device__ __forceinline__ void agg_edges(const GatAgg& p, int beg, int end, int
     for (int u = 0; u < U; ++u) {
       const int kk = k0 + u;
       if (kk < end) {
-        const V* row = F + (size_t)__ldg(p.col + kk) * ldv + lane;
+        const int c = __ldg(p.col + kk);
+        const V* row = F + (size_t)c * ldv + lane;
         const float* ak = p.a + (size_t)(p.eidx ? __ldg(p.eidx + kk) : kk) * p.H;
+        float ss = 1.f;
+        if (SS) ss = src_scale ? __ldg(src_scale + c) : 1.f;
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
-          if (lane + 32 * j < nvec) { x[u][j] = vldg(row + 32 * j); w[u][j] = __ldg(ak + head[j]); }
+          if (lane + 32 * j < nvec) { x[u][j] = vldg(row + 32 * j); w[u][j] = SS ? __ldg(ak + head[j]) * ss : __ldg(ak + head[j]); }
           else { vzero(x[u][j]); w[u][j] = 0.f; }
         }
       } else {
@@ -496,6 +500,209 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_bwd_hub_finalize_kernel(const
   }
 }
 
+// ---------------------------------------------------------------- aggregate with the layer's epilogue
+// The fused GAT layer (engine_gat.py): out[i,:] = row_scale[i] * sum_k a[k,h] src_scale[col[k]] ft[col[k],h,:] + res[i,:] + bias,
+// and per CTA the (sum, sum of squares) of its output rows in the [slots][2][K] layout b200gnn_bn_finalize_f32 reads.
+// Same decomposition and summation order as gat_aggregate_kernel: with every epilogue operand absent the output is its
+// output bit for bit (a * 1.f is a).
+struct GatEpi {
+  const float* src_scale; const float* row_scale; const float* res; const float* bias; float* stat;
+  int64_t ldr; int32_t n_main;   // n_main: CTAs of the chunk part of the launch = first hub slot
+};
+
+template <typename V>
+__device__ __forceinline__ V epi_row(const GatEpi& q, V y, int64_t r, int v) {
+  constexpr int W = VecTraits<V>::W;
+  if (q.row_scale) { V z; vzero(z); vfma(z, __ldg(q.row_scale + r), y); y = z; }
+  if (q.res) vadd(y, vldg(reinterpret_cast<const V*>(q.res + (size_t)r * q.ldr) + v));
+  if (q.bias) vadd(y, vldg(reinterpret_cast<const V*>(q.bias) + v));
+  (void)W;
+  return y;
+}
+
+template <typename V, int NJ, int U>
+__global__ void __launch_bounds__(GAT_THREADS) gat_aggregate_epi_kernel(const GatAgg p, const GatEpi q) {
+  constexpr int W = VecTraits<V>::W;
+  extern __shared__ float s_row[];   // K floats (hub-segment CTAs), 2K floats (statistics of the chunk CTAs)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nvec = p.K / W;
+  int head[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) head[j] = ((lane + 32 * j) * W) / p.D;
+  if ((int)blockIdx.x < p.n_seg) {
+    int r, b, e;
+    hub_segment(p.rowptr, p.hub_rows, p.hub_segptr, p.n_hub, p.seg_len, blockIdx.x, r, b, e);
+    V acc[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) vzero(acc[j]);
+    agg_edges<V, NJ, U, true>(p, b, e, warp, GAT_WARPS, lane, nvec, head, acc, q.src_scale);
+    for (int i = threadIdx.x; i < p.K; i += GAT_THREADS) s_row[i] = 0.f;
+    __syncthreads();
+    V* sv = reinterpret_cast<V*>(s_row);
+    for (int w = 0; w < GAT_WARPS; ++w) {
+      if (warp == w) {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+          if (lane + 32 * j < nvec) { V t = sv[lane + 32 * j]; vadd(t, acc[j]); sv[lane + 32 * j] = t; }
+      }
+      __syncthreads();
+    }
+    for (int i = threadIdx.x; i < p.K; i += GAT_THREADS) p.ws[(size_t)blockIdx.x * p.K + i] = s_row[i];
+    return;
+  }
+  V* O = reinterpret_cast<V*>(p.out);
+  const size_t ldov = (size_t)(p.ldo / W);
+  const int cta = blockIdx.x - p.n_seg;
+  const int chunk = cta * GAT_WARPS + warp;
+  V ssum[NJ], ssq[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { vzero(ssum[j]); vzero(ssq[j]); }
+  if (chunk < p.n_chunks) {
+    const int r0 = __ldg(p.chunk_rowptr + chunk), r1 = __ldg(p.chunk_rowptr + chunk + 1);
+    for (int r = r0; r < r1; ++r) {
+      const int b = __ldg(p.rowptr + r), e = __ldg(p.rowptr + r + 1);
+      if (e - b > p.hub_threshold) continue;
+      V acc[NJ];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) vzero(acc[j]);
+      agg_edges<V, NJ, U, true>(p, b, e, 0, 1, lane, nvec, head, acc, q.src_scale);
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+        if (lane + 32 * j < nvec) {
+          const V y = epi_row<V>(q, acc[j], r, lane + 32 * j);
+          O[(size_t)r * ldov + lane + 32 * j] = y;
+          if (q.stat) vstat(ssum[j], ssq[j], y);
+        }
+    }
+  }
+  if (q.stat) {     // the CTA's warps combine in warp order; every slot is written on every launch
+    for (int i = threadIdx.x; i < 2 * p.K; i += GAT_THREADS) s_row[i] = 0.f;
+    __syncthreads();
+    V* ss = reinterpret_cast<V*>(s_row);
+    V* sq = reinterpret_cast<V*>(s_row + p.K);
+    for (int w = 0; w < GAT_WARPS; ++w) {
+      if (warp == w) {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+          if (lane + 32 * j < nvec) {
+            V t = ss[lane + 32 * j]; vadd(t, ssum[j]); ss[lane + 32 * j] = t;
+            V u = sq[lane + 32 * j]; vadd(u, ssq[j]); sq[lane + 32 * j] = u;
+          }
+      }
+      __syncthreads();
+    }
+    float* out = q.stat + (size_t)cta * 2 * p.K;
+    for (int i = threadIdx.x; i < 2 * p.K; i += GAT_THREADS) out[i] = s_row[i];
+  }
+}
+
+__global__ void __launch_bounds__(GAT_THREADS) gat_hub_finalize_epi_kernel(const int32_t* __restrict__ hub_rows,
+                                                                           const int32_t* __restrict__ hub_segptr,
+                                                                           const float* __restrict__ ws, float* __restrict__ out,
+                                                                           int64_t ldo, int K, const GatEpi q) {
+  const int r = __ldg(hub_rows + blockIdx.x);
+  const int q0 = __ldg(hub_segptr + blockIdx.x), q1 = __ldg(hub_segptr + blockIdx.x + 1);
+  float* stat = q.stat ? q.stat + (size_t)(q.n_main + blockIdx.x) * 2 * K : nullptr;
+  for (int i = threadIdx.x; i < K; i += GAT_THREADS) {
+    float t = 0.f;
+    for (int s = q0; s < q1; ++s) t += ws[(size_t)s * K + i];
+    t = epi_row<float>(q, t, r, i);
+    out[(size_t)r * ldo + i] = t;
+    if (stat) { stat[i] = t; stat[K + i] = t * t; }
+  }
+}
+
+// ---------------------------------------------------------------- attention scores
+// el[n,h] = src_scale[n] * <ft[n,h,:], attn_l[h,:]>,  er[n,h] = <ft[n,h,:], attn_r[h,:]>   (one warp per node; lanes
+// stride over the head and combine by the xor butterfly: one fixed order)
+struct GatScores {
+  const float* ft; const float* attn_l; const float* attn_r; const float* src_scale; float* el; float* er;
+  int64_t ldf, n_rows; int32_t H, D;
+};
+
+__global__ void __launch_bounds__(GAT_THREADS) gat_scores_kernel(const GatScores p) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int64_t n = (int64_t)blockIdx.x * GAT_WARPS + warp; n < p.n_rows; n += (int64_t)gridDim.x * GAT_WARPS) {
+    const float* row = p.ft + (size_t)n * p.ldf;
+    const float sc = p.src_scale ? __ldg(p.src_scale + n) : 1.f;
+    for (int h = 0; h < p.H; ++h) {
+      float sl = 0.f, sr = 0.f;
+      for (int d = lane; d < p.D; d += 32) {
+        const float f = __ldg(row + h * p.D + d);
+        sl = fmaf(f, __ldg(p.attn_l + h * p.D + d), sl);
+        if (p.attn_r) sr = fmaf(f, __ldg(p.attn_r + h * p.D + d), sr);
+      }
+      sl = gsum(sl);
+      if (p.attn_r) sr = gsum(sr);
+      if (lane == 0) {
+        p.el[(size_t)n * p.H + h] = p.src_scale ? sl * sc : sl;
+        if (p.attn_r) p.er[(size_t)n * p.H + h] = sr;
+      }
+    }
+  }
+}
+
+// backward: dft[n,h,:] += del[n,h] src_scale[n] attn_l[h,:] + der[n,h] attn_r[h,:] in place, and per CTA (a contiguous
+// block of rows, added in row order) the partial sums of d attn_l / d attn_r; a second kernel adds the slots in order.
+constexpr int GAT_SB_MAXJ = 6;   // columns per thread: K <= 1536
+struct GatScoresBwd {
+  const float* ft; const float* attn_l; const float* attn_r; const float* src_scale; const float* del; const float* der;
+  float* dft; float* partial;   // [slots][2][K]
+  int64_t ldf, ldd, n_rows; int32_t H, D, K, rows_per_cta;
+};
+
+__global__ void __launch_bounds__(GAT_THREADS) gat_scores_bwd_kernel(const GatScoresBwd p) {
+  float al[GAT_SB_MAXJ], ar[GAT_SB_MAXJ], accl[GAT_SB_MAXJ], accr[GAT_SB_MAXJ];
+  int hd[GAT_SB_MAXJ];
+#pragma unroll
+  for (int j = 0; j < GAT_SB_MAXJ; ++j) {
+    const int k = threadIdx.x + GAT_THREADS * j;
+    hd[j] = k < p.K ? k / p.D : 0;
+    al[j] = k < p.K ? __ldg(p.attn_l + k) : 0.f;
+    ar[j] = (k < p.K && p.attn_r) ? __ldg(p.attn_r + k) : 0.f;
+    accl[j] = accr[j] = 0.f;
+  }
+  const int64_t r0 = (int64_t)blockIdx.x * p.rows_per_cta;
+  const int64_t r1 = r0 + p.rows_per_cta < p.n_rows ? r0 + p.rows_per_cta : p.n_rows;
+  for (int64_t n = r0; n < r1; ++n) {
+    const float sc = p.src_scale ? __ldg(p.src_scale + n) : 1.f;
+#pragma unroll
+    for (int j = 0; j < GAT_SB_MAXJ; ++j) {
+      const int k = threadIdx.x + GAT_THREADS * j;
+      if (k < p.K) {
+        const float gl = __ldg(p.del + (size_t)n * p.H + hd[j]) * sc;
+        const float f = __ldg(p.ft + (size_t)n * p.ldf + k);
+        float g = fmaf(gl, al[j], p.dft[(size_t)n * p.ldd + k]);
+        accl[j] = fmaf(gl, f, accl[j]);
+        if (p.attn_r) {
+          const float gr = __ldg(p.der + (size_t)n * p.H + hd[j]);
+          g = fmaf(gr, ar[j], g);
+          accr[j] = fmaf(gr, f, accr[j]);
+        }
+        p.dft[(size_t)n * p.ldd + k] = g;
+      }
+    }
+  }
+  float* out = p.partial + (size_t)blockIdx.x * 2 * p.K;
+#pragma unroll
+  for (int j = 0; j < GAT_SB_MAXJ; ++j) {
+    const int k = threadIdx.x + GAT_THREADS * j;
+    if (k < p.K) { out[k] = accl[j]; out[p.K + k] = accr[j]; }
+  }
+}
+
+__global__ void __launch_bounds__(GAT_THREADS) gat_scores_bwd_finalize_kernel(const float* __restrict__ partial, int slots, int K,
+                                                                              float* __restrict__ d_attn_l,
+                                                                              float* __restrict__ d_attn_r) {
+  const int i = blockIdx.x * GAT_THREADS + threadIdx.x;
+  if (i >= 2 * K) return;
+  float* dst = i < K ? d_attn_l + i : (d_attn_r ? d_attn_r + (i - K) : nullptr);
+  if (!dst) return;
+  float t = 0.f;
+  for (int s = 0; s < slots; ++s) t += partial[(size_t)s * 2 * K + i];
+  *dst = t;
+}
+
 static inline int rows_grid(int64_t n) {
   int64_t g = (n + GAT_WARPS - 1) / GAT_WARPS;
   if (g > 132 * 16) g = 132 * 16;
@@ -513,6 +720,36 @@ static int launch_agg_nj(const GatAgg& p, cudaStream_t st) {
     if ((rc = check_launch())) return rc;
   }
   return B200GNN_OK;
+}
+
+template <typename V, int NJ, int U>
+static int launch_agg_epi_nj(const GatAgg& p, const GatEpi& q0, cudaStream_t st) {
+  int rc;
+  GatEpi q = q0;
+  q.n_main = (p.n_chunks + GAT_WARPS - 1) / GAT_WARPS;
+  const int grid = p.n_seg + q.n_main;
+  const size_t smem = (q.stat ? 2 * p.K : (p.n_seg > 0 ? p.K : 0)) * sizeof(float);
+  gat_aggregate_epi_kernel<V, NJ, U><<<grid, GAT_THREADS, smem, st>>>(p, q);
+  if ((rc = check_launch())) return rc;
+  if (p.n_hub > 0) {
+    gat_hub_finalize_epi_kernel<<<p.n_hub, GAT_THREADS, 0, st>>>(p.hub_rows, p.hub_segptr, p.ws, p.out, p.ldo, p.K, q);
+    if ((rc = check_launch())) return rc;
+  }
+  return B200GNN_OK;
+}
+template <typename V>
+static int launch_agg_epi(const GatAgg& p, const GatEpi& q, cudaStream_t st) {   // the (NJ, U) choice of launch_agg
+  constexpr int W = VecTraits<V>::W;
+  const int nj = (p.K / W + 31) / 32;
+  if constexpr (W == 4) {
+    if (nj <= 1) return launch_agg_epi_nj<V, 1, 8>(p, q, st);
+    if (nj <= 2) return launch_agg_epi_nj<V, 2, 4>(p, q, st);
+  }
+  if (nj <= 4) return launch_agg_epi_nj<V, 4, 2>(p, q, st);
+  if constexpr (W == 4) {
+    if (nj <= 8) return launch_agg_epi_nj<V, 8, 1>(p, q, st);
+  }
+  return launch_agg_epi_nj<V, GAT_MAXJ, 1>(p, q, st);
 }
 
 template <typename V, int NJ, int U, bool SEG>
@@ -649,5 +886,89 @@ extern "C" int b200gnn_segment_sum_heads_f32(const int32_t* rowptr, const int32_
   GatSegSum p;
   p.rowptr = rowptr; p.eidx = eidx; p.vals = vals; p.out = out; p.n_rows = n_rows; p.H = (int32_t)H;
   gat_segment_sum_kernel<<<rows_grid(n_rows), GAT_THREADS, 0, (cudaStream_t)stream>>>(p);
+  return check_launch();
+}
+
+// ---- the fused GAT layer (engine_gat.py)
+extern "C" int64_t b200gnn_gat_stat_slots(int64_t n_chunks, int64_t n_hub) {
+  if (n_chunks < 0 || n_hub < 0) return B200GNN_ERR_BAD_ARG;
+  return (n_chunks + GAT_WARPS - 1) / GAT_WARPS + n_hub;
+}
+
+extern "C" int b200gnn_gat_aggregate_epi_f32(const int32_t* rowptr, const int32_t* col, const int32_t* eidx, const float* a,
+                                             const float* ft, int64_t ldf, float* out, int64_t ldo, int64_t n_rows, int64_t H,
+                                             int64_t D, const float* src_scale, const float* row_scale, const float* res,
+                                             int64_t ldr, const float* bias, float* stat_partial, int64_t stat_slots,
+                                             const int32_t* chunk_rowptr, int64_t n_chunks, int32_t hub_threshold,
+                                             int32_t seg_len, const int32_t* hub_rows, const int32_t* hub_segptr, int64_t n_hub,
+                                             int64_t n_seg, float* hub_workspace, void* stream) {
+  const int64_t K = H * D;
+  if (!rowptr || !a || !ft || !out || n_rows < 0 || H <= 0 || D <= 0 || H > GAT_MAXH || ldf < K || ldo < K || !chunk_rowptr ||
+      n_chunks < 0 || n_hub < 0 || n_seg < n_hub || (res && ldr < K) ||
+      (stat_partial && stat_slots < b200gnn_gat_stat_slots(n_chunks, n_hub)) ||
+      (n_hub > 0 && (!hub_rows || !hub_segptr || !hub_workspace || seg_len <= 0)))
+    return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0 || n_chunks == 0) return B200GNN_OK;
+  GatAgg p;
+  p.rowptr = rowptr; p.col = col; p.eidx = eidx; p.chunk_rowptr = chunk_rowptr; p.hub_rows = hub_rows;
+  p.hub_segptr = hub_segptr; p.ws = hub_workspace;
+  p.a = a; p.ft = ft; p.out = out; p.ldf = ldf; p.ldo = ldo;
+  p.n_chunks = (int32_t)n_chunks; p.n_hub = (int32_t)n_hub; p.n_seg = (int32_t)(n_hub > 0 ? n_seg : 0); p.seg_len = seg_len;
+  p.hub_threshold = hub_threshold;
+  p.H = (int32_t)H; p.D = (int32_t)D; p.K = (int32_t)K;
+  GatEpi q;
+  q.src_scale = src_scale; q.row_scale = row_scale; q.res = res; q.bias = bias; q.stat = stat_partial; q.ldr = res ? ldr : 0;
+  q.n_main = 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool r4 = !res || (ldr % 4 == 0 && aligned_to(res, 16)), r2 = !res || (ldr % 2 == 0 && aligned_to(res, 8));
+  const bool b4 = !bias || aligned_to(bias, 16), b2 = !bias || aligned_to(bias, 8);
+  if (D % 4 == 0 && ldf % 4 == 0 && ldo % 4 == 0 && aligned_to(ft, 16) && aligned_to(out, 16) && r4 && b4 && K <= 4 * 32 * GAT_MAXJ)
+    return launch_agg_epi<float4>(p, q, st);
+  if (D % 2 == 0 && ldf % 2 == 0 && ldo % 2 == 0 && aligned_to(ft, 8) && aligned_to(out, 8) && r2 && b2 && K <= 2 * 32 * GAT_MAXJ)
+    return launch_agg_epi<float2>(p, q, st);
+  if (K <= 32 * GAT_MAXJ) return launch_agg_epi<float>(p, q, st);
+  return B200GNN_ERR_UNSUPPORTED;
+}
+
+extern "C" int b200gnn_gat_scores_f32(const float* ft, int64_t ldf, const float* attn_l, const float* attn_r,
+                                      const float* src_scale, int64_t n_rows, int64_t H, int64_t D, float* el, float* er,
+                                      void* stream) {
+  if (!ft || !attn_l || !el || (attn_r && !er) || n_rows < 0 || H <= 0 || D <= 0 || H > GAT_MAXH || ldf < H * D)
+    return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  GatScores p;
+  p.ft = ft; p.attn_l = attn_l; p.attn_r = attn_r; p.src_scale = src_scale; p.el = el; p.er = er; p.ldf = ldf; p.n_rows = n_rows;
+  p.H = (int32_t)H; p.D = (int32_t)D;
+  gat_scores_kernel<<<rows_grid(n_rows), GAT_THREADS, 0, (cudaStream_t)stream>>>(p);
+  return check_launch();
+}
+
+// slots of the [slots][2][H*D] partial buffer of b200gnn_gat_scores_bwd_f32
+extern "C" int64_t b200gnn_gat_scores_slots(int64_t n_rows) {
+  if (n_rows < 0) return B200GNN_ERR_BAD_ARG;
+  const int64_t s = (n_rows + 63) / 64;
+  return s < 1 ? 1 : (s > 132 * 4 ? 132 * 4 : s);
+}
+
+extern "C" int b200gnn_gat_scores_bwd_f32(const float* ft, int64_t ldf, const float* attn_l, const float* attn_r,
+                                          const float* src_scale, const float* d_el, const float* d_er, int64_t n_rows,
+                                          int64_t H, int64_t D, float* dft, int64_t ldd, float* d_attn_l, float* d_attn_r,
+                                          float* partial, int64_t slots, void* stream) {
+  const int64_t K = H * D;
+  if (!ft || !attn_l || !d_el || !dft || !d_attn_l || !partial || (attn_r && (!d_er || !d_attn_r)) || n_rows <= 0 || H <= 0 ||
+      D <= 0 || H > GAT_MAXH || ldf < K || ldd < K || slots < b200gnn_gat_scores_slots(n_rows))
+    return B200GNN_ERR_BAD_ARG;
+  if (K > GAT_THREADS * GAT_SB_MAXJ) return B200GNN_ERR_UNSUPPORTED;
+  const int64_t used = b200gnn_gat_scores_slots(n_rows);
+  GatScoresBwd p;
+  p.ft = ft; p.attn_l = attn_l; p.attn_r = attn_r; p.src_scale = src_scale; p.del = d_el; p.der = d_er; p.dft = dft;
+  p.partial = partial; p.ldf = ldf; p.ldd = ldd; p.n_rows = n_rows; p.H = (int32_t)H; p.D = (int32_t)D; p.K = (int32_t)K;
+  p.rows_per_cta = (int32_t)((n_rows + used - 1) / used);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  gat_scores_bwd_kernel<<<(int)used, GAT_THREADS, 0, st>>>(p);
+  if ((rc = check_launch())) return rc;
+  gat_scores_bwd_finalize_kernel<<<(int)((2 * K + GAT_THREADS - 1) / GAT_THREADS), GAT_THREADS, 0, st>>>(
+      partial, (int)used, (int)K, d_attn_l, attn_r ? d_attn_r : nullptr);
   return check_launch();
 }

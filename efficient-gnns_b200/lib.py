@@ -56,6 +56,7 @@ SIGNATURES = {
     "b200gnn_affine_relu_dropout_scatter_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32p, _f32p, _int, _f32, _u64, _u64,
                                                        _i32p, _u64, _i32p, _u64, _i64, _i64, _ptr, _ptr, _i32, _i64, _ptr]),
     "b200gnn_dropout_mask_u8": (_int, [_ptr, _i64, _i64, _f32, _u64, _u64, _ptr]),
+    "b200gnn_dropout_mask_step_u8": (_int, [_ptr, _i64, _i64, _f32, _u64, _u64, _i32p, _u64, _ptr]),
     "b200gnn_dropout_bits_u32": (_int, [_ptr, _i64, _i64, _i64, _f32, _u64, _u64, _i32p, _u64, _ptr]),
     "b200gnn_affine_relu_bits_f32": (_int, [_f32p, _ptr, _f32p, _f32p, _f32, _f32p, _i64, _i64, _ptr]),
     "b200gnn_relu_dropout_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _ptr]),
@@ -127,6 +128,14 @@ SIGNATURES = {
     "b200gnn_gat_bwd_rows_f32": (_int, [_i32p, _i32p, _f32p, _f32p, _i64, _f32p, _i64, _f32p, _f32p, _i64, _i64, _i64, _f32,
                                         _f32p, _f32p, _i32p, _i64, _i32, _i32, _i32p, _i32p, _i64, _i64, _f32p, _f32p, _ptr]),
     "b200gnn_segment_sum_heads_f32": (_int, [_i32p, _i32p, _f32p, _i64, _i64, _f32p, _ptr]),
+    "b200gnn_gat_scores_f32": (_int, [_f32p, _i64, _f32p, _f32p, _f32p, _i64, _i64, _i64, _f32p, _f32p, _ptr]),
+    "b200gnn_gat_scores_slots": (_i64, [_i64]),
+    "b200gnn_gat_scores_bwd_f32": (_int, [_f32p, _i64, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _i64, _f32p, _i64,
+                                          _f32p, _f32p, _f32p, _i64, _ptr]),
+    "b200gnn_gat_stat_slots": (_i64, [_i64, _i64]),
+    "b200gnn_gat_aggregate_epi_f32": (_int, [_i32p, _i32p, _i32p, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64,
+                                             _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _i64, _i32p, _i64, _i32, _i32,
+                                             _i32p, _i32p, _i64, _i64, _f32p, _ptr]),
     "b200gnn_graph_sort_workspace_bytes": (_i64, [_i64]),
     "b200gnn_graph_argsort_i64": (_int, [_ptr, _ptr, _i64, _i64, _i64, _i32p, _ptr, _ptr]),
     "b200gnn_graph_coalesce_i64": (_int, [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _i32p, _ptr, _ptr, _ptr, _ptr]),

@@ -724,3 +724,73 @@ def sign_gather(feats, idx: torch.Tensor, p: float, seed: int, offset: int, out:
         _f32(teacher, "teacher"), teacher.stride(0) if teacher is not None else 0, C, _f32(teacher_out, "teacher_out"),
         lib.stream_ptr()), "sign_gather_f32")
     return out
+
+
+# ----------------------------------------------------------------------------- fused GAT layer (engine_gat.py)
+def dropout_mask_step(mask: torch.Tensor, p: float, seed: int, offset: int, step_dev: torch.Tensor, step_mul: int) -> torch.Tensor:
+    """Fill the flat uint8 ``mask`` (a multiple of 4 elements) with the decisions of ``dropout_mask`` for the effective offset
+    offset + step_dev * step_mul, read on the device."""
+    assert mask.dtype == torch.uint8 and mask.is_contiguous() and mask.numel() % 4 == 0
+    lib.check(lib.load().b200gnn_dropout_mask_step_u8(mask.data_ptr(), mask.numel() // 4, 4, p, seed, offset,
+                                                      lib.dptr(step_dev, torch.int32, "step_dev"), step_mul, lib.stream_ptr()),
+              "dropout_mask_step_u8")
+    return mask
+
+
+def gat_scores(ft: torch.Tensor, attn_l: torch.Tensor, attn_r: Optional[torch.Tensor], src_scale: Optional[torch.Tensor],
+               H: int, el: Optional[torch.Tensor] = None, er: Optional[torch.Tensor] = None):
+    """el[n,h] = src_scale[n]·<ft[n,h,:], attn_l[h,:]>, er[n,h] = <ft[n,h,:], attn_r[h,:]>; ft [N, H*D] may be a column block."""
+    n, K = ft.shape
+    fp, ldf = _rows(ft, "ft")
+    el = torch.empty(n, H, dtype=torch.float32, device=ft.device) if el is None else el
+    if attn_r is not None and er is None:
+        er = torch.empty(n, H, dtype=torch.float32, device=ft.device)
+    lib.check(lib.load().b200gnn_gat_scores_f32(fp, ldf, _f32(attn_l, "attn_l"), _f32(attn_r, "attn_r"), _f32(src_scale, "src_scale"),
+                                                n, H, K // H, _f32(el, "el"), _f32(er, "er") if attn_r is not None else None,
+                                                lib.stream_ptr()), "gat_scores_f32")
+    return el, (er if attn_r is not None else None)
+
+
+def gat_scores_slots(n_rows: int) -> int:
+    return int(lib.load().b200gnn_gat_scores_slots(n_rows))
+
+
+def gat_scores_bwd(ft: torch.Tensor, attn_l: torch.Tensor, attn_r: Optional[torch.Tensor], src_scale: Optional[torch.Tensor],
+                   d_el: torch.Tensor, d_er: Optional[torch.Tensor], H: int, dft: torch.Tensor, d_attn_l: torch.Tensor,
+                   d_attn_r: Optional[torch.Tensor], partial: Optional[torch.Tensor] = None) -> None:
+    """dft += d_el·src_scale·attn_l + d_er·attn_r in place; d_attn_l / d_attn_r reduced through per-CTA partials in slot order."""
+    n, K = ft.shape
+    fp, ldf = _rows(ft, "ft")
+    dp, ldd = _rows(dft, "dft")
+    if partial is None:
+        partial = torch.empty(gat_scores_slots(n), 2, K, dtype=torch.float32, device=ft.device)
+    lib.check(lib.load().b200gnn_gat_scores_bwd_f32(
+        fp, ldf, _f32(attn_l, "attn_l"), _f32(attn_r, "attn_r"), _f32(src_scale, "src_scale"), _f32(d_el, "d_el"),
+        _f32(d_er, "d_er") if attn_r is not None else None, n, H, K // H, dp, ldd, _f32(d_attn_l, "d_attn_l"),
+        _f32(d_attn_r, "d_attn_r") if attn_r is not None else None, _f32(partial, "partial"), partial.shape[0],
+        lib.stream_ptr()), "gat_scores_bwd_f32")
+
+
+def gat_stat_slots(g: CsrGraph) -> int:
+    return int(lib.load().b200gnn_gat_stat_slots(g.n_chunks, g.n_hub))
+
+
+def gat_aggregate_epi(g: CsrGraph, eidx: Optional[torch.Tensor], a: torch.Tensor, ft: torch.Tensor, out: torch.Tensor, H: int,
+                      src_scale: Optional[torch.Tensor] = None, row_scale: Optional[torch.Tensor] = None,
+                      res: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None,
+                      stat_partial: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[i] = row_scale[i]·Σ_e a[e,h]·src_scale[col[e]]·ft[col[e],h,:] + res[i] + bias, with the BatchNorm partial sums of the
+    output rows in stat_partial [gat_stat_slots(g), 2, K]; ft / res / out may be column blocks.  No operands: gat_aggregate."""
+    K = ft.shape[1]
+    fp, ldf = _rows(ft, "ft")
+    op, ldo = _rows(out, "out")
+    rp, ldr = _rows(res, "res") if res is not None else (None, 0)
+    ws = g.hub_workspace(K)
+    lib.check(lib.load().b200gnn_gat_aggregate_epi_f32(
+        g.rowptr.data_ptr(), g.col.data_ptr(), lib.dptr(eidx, torch.int32, "eidx"), _f32(a, "a"), fp, ldf, op, ldo, g.n_rows, H,
+        K // H, _f32(src_scale, "src_scale"), _f32(row_scale, "row_scale"), rp, ldr, _f32(bias, "bias"),
+        _f32(stat_partial, "stat_partial"), 0 if stat_partial is None else stat_partial.shape[0],
+        g.chunk_rowptr.data_ptr(), g.n_chunks, g.hub_threshold, g.seg_len,
+        g.hub_rows.data_ptr() if g.n_hub else None, g.hub_segptr.data_ptr() if g.n_hub else None, g.n_hub, g.n_seg,
+        None if ws is None else ws.data_ptr(), lib.stream_ptr()), "gat_aggregate_epi_f32")
+    return out

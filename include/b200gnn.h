@@ -187,6 +187,10 @@ int b200gnn_affine_relu_dropout_scatter_f32(const float* Y, float* out, int64_t 
                                             const int32_t* row_off, int32_t world, int64_t ld_dst, void* stream);
 int b200gnn_dropout_mask_u8(uint8_t* mask, int64_t n_rows, int64_t K, float p,
                             uint64_t seed, uint64_t offset, void* stream);
+/* b200gnn_dropout_mask_u8 of the effective offset offset + *step_dev * step_mul, read on the device: the edge keep-mask of
+ * the GAT step's edge drop (arxiv_dgl/models.py:207-212), fresh on every replay of a captured graph. */
+int b200gnn_dropout_mask_step_u8(uint8_t* mask, int64_t n_rows, int64_t K, float p, uint64_t seed, uint64_t offset,
+                                 const int32_t* step_dev, uint64_t step_mul, void* stream);
 /* The keep decisions of b200gnn_affine_relu_dropout_f32 (row_offset 0) packed one bit per element, for n_layers
  * [n_rows, K] activations in one launch: layer l uses effective offset offset + l (+ *step_dev * step_mul) and fills
  * bits[l][row][w], w < ceil(K/32), bit b = column 32 w + b (bits past K are zero).  Needs no input: it can run next to
@@ -515,6 +519,43 @@ int b200gnn_gat_bwd_rows_f32(const int32_t* rowptr, const int32_t* col, const fl
 int b200gnn_segment_sum_heads_f32(const int32_t* rowptr, const int32_t* eidx,
                                   const float* vals, int64_t n_rows, int64_t H,
                                   float* out, void* stream);
+
+/* ------------------------------------------------------------------ *
+ * The fused GAT layer of the full-batch trainer (engine_gat.py): what the reference's GATConv.forward runs as separate
+ * [N, H*D] torch ops around its two DGL kernels.
+ *   gat_scores        : el[n,h] = src_scale[n] * <ft[n,h,:], attn_l[h,:]>, er[n,h] = <ft[n,h,:], attn_r[h,:]> in one read of
+ *                       ft (row pitch ldf) — arxiv_dgl/models.py:179-184 (feat_src * out_deg^-1/2), :196 (el), :200 (er from
+ *                       the un-normalised projection).  src_scale / attn_r (with er) may be NULL.  One warp per node, fixed
+ *                       summation order.
+ *   gat_scores_bwd    : dft[n,h,:] += d_el[n,h] src_scale[n] attn_l[h,:] + d_er[n,h] attn_r[h,:] in place, d_attn_l[h,:] =
+ *                       sum_n d_el[n,h] src_scale[n] ft[n,h,:], d_attn_r[h,:] = sum_n d_er[n,h] ft[n,h,:] (autograd of
+ *                       models.py:196,200): per-CTA partials over contiguous row blocks (partial: [slots][2][H*D] floats,
+ *                       slots >= b200gnn_gat_scores_slots(n_rows)) added in slot order — no atomics, repeatable.  H*D <= 1536.
+ *   gat_aggregate_epi : b200gnn_gat_aggregate_f32 (same plans, same summation order) with the rest of the layer in its
+ *                       epilogue: out[i,:] = row_scale[i] * sum_e a[e,h] src_scale[col[e]] ft[col[e],h,:] + res[i,:] + bias
+ *                       (models.py:184 folded into the coefficient, :220-225 in_deg^+1/2, :228-230 residual, :311
+ *                       bias_last), and stat_partial[slots][2][H*D] = per-CTA (sum, sum of squares) of the output rows,
+ *                       slots >= b200gnn_gat_stat_slots(n_chunks, n_hub), the input of b200gnn_bn_finalize_f32
+ *                       (models.py:304's BatchNorm1d statistics).  Every epilogue operand may be NULL; with all of them
+ *                       NULL the output equals b200gnn_gat_aggregate_f32's bit for bit.  Run on the transposed graph with
+ *                       the two scale vectors exchanged it is the backward aggregation (d ft).
+ * ------------------------------------------------------------------ */
+int b200gnn_gat_scores_f32(const float* ft, int64_t ldf, const float* attn_l, const float* attn_r,
+                           const float* src_scale, int64_t n_rows, int64_t H, int64_t D, float* el, float* er,
+                           void* stream);
+int64_t b200gnn_gat_scores_slots(int64_t n_rows);
+int b200gnn_gat_scores_bwd_f32(const float* ft, int64_t ldf, const float* attn_l, const float* attn_r,
+                               const float* src_scale, const float* d_el, const float* d_er, int64_t n_rows,
+                               int64_t H, int64_t D, float* dft, int64_t ldd, float* d_attn_l, float* d_attn_r,
+                               float* partial, int64_t slots, void* stream);
+int64_t b200gnn_gat_stat_slots(int64_t n_chunks, int64_t n_hub);
+int b200gnn_gat_aggregate_epi_f32(const int32_t* rowptr, const int32_t* col, const int32_t* eidx, const float* a,
+                                  const float* ft, int64_t ldf, float* out, int64_t ldo, int64_t n_rows, int64_t H,
+                                  int64_t D, const float* src_scale, const float* row_scale, const float* res,
+                                  int64_t ldr, const float* bias, float* stat_partial, int64_t stat_slots,
+                                  const int32_t* chunk_rowptr, int64_t n_chunks, int32_t hub_threshold,
+                                  int32_t seg_len, const int32_t* hub_rows, const int32_t* hub_segptr, int64_t n_hub,
+                                  int64_t n_seg, float* hub_workspace, void* stream);
 
 /* ------------------------------------------------------------------
  * Peer-memory exchange of the node-parallel engine (SURVEY.md §8e; no reference counterpart: the reference is
