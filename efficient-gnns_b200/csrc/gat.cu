@@ -507,7 +507,8 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_bwd_hub_finalize_kernel(const
 // output bit for bit (a * 1.f is a).
 struct GatEpi {
   const float* src_scale; const float* row_scale; const float* res; const float* bias; float* stat;
-  int64_t ldr; int32_t n_main;   // n_main: CTAs of the chunk part of the launch = first hub slot
+  float* act;                    // ELU instantiations only: elu(out) is also stored here, row pitch lda
+  int64_t ldr, lda; int32_t n_main;   // n_main: CTAs of the chunk part of the launch = first hub slot
 };
 
 template <typename V>
@@ -520,7 +521,13 @@ __device__ __forceinline__ V epi_row(const GatEpi& q, V y, int64_t r, int v) {
   return y;
 }
 
-template <typename V, int NJ, int U>
+// F.elu with alpha 1 as torch computes it: z > 0 ? z : expm1(z)
+__device__ __forceinline__ float elu1(float z) { return z > 0.f ? z : expm1f(z); }
+__device__ __forceinline__ float velu(float z) { return elu1(z); }
+__device__ __forceinline__ float2 velu(float2 z) { return make_float2(elu1(z.x), elu1(z.y)); }
+__device__ __forceinline__ float4 velu(float4 z) { return make_float4(elu1(z.x), elu1(z.y), elu1(z.z), elu1(z.w)); }
+
+template <typename V, int NJ, int U, bool ELU = false>
 __global__ void __launch_bounds__(GAT_THREADS) gat_aggregate_epi_kernel(const GatAgg p, const GatEpi q) {
   constexpr int W = VecTraits<V>::W;
   extern __shared__ float s_row[];   // K floats (hub-segment CTAs), 2K floats (statistics of the chunk CTAs)
@@ -571,6 +578,7 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_aggregate_epi_kernel(const Ga
         if (lane + 32 * j < nvec) {
           const V y = epi_row<V>(q, acc[j], r, lane + 32 * j);
           O[(size_t)r * ldov + lane + 32 * j] = y;
+          if (ELU) reinterpret_cast<V*>(q.act)[(size_t)r * (size_t)(q.lda / W) + lane + 32 * j] = velu(y);
           if (q.stat) vstat(ssum[j], ssq[j], y);
         }
     }
@@ -596,6 +604,7 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_aggregate_epi_kernel(const Ga
   }
 }
 
+template <bool ELU = false>
 __global__ void __launch_bounds__(GAT_THREADS) gat_hub_finalize_epi_kernel(const int32_t* __restrict__ hub_rows,
                                                                            const int32_t* __restrict__ hub_segptr,
                                                                            const float* __restrict__ ws, float* __restrict__ out,
@@ -608,6 +617,7 @@ __global__ void __launch_bounds__(GAT_THREADS) gat_hub_finalize_epi_kernel(const
     for (int s = q0; s < q1; ++s) t += ws[(size_t)s * K + i];
     t = epi_row<float>(q, t, r, i);
     out[(size_t)r * ldo + i] = t;
+    if (ELU) q.act[(size_t)r * q.lda + i] = elu1(t);
     if (stat) { stat[i] = t; stat[K + i] = t * t; }
   }
 }
@@ -722,34 +732,34 @@ static int launch_agg_nj(const GatAgg& p, cudaStream_t st) {
   return B200GNN_OK;
 }
 
-template <typename V, int NJ, int U>
+template <typename V, int NJ, int U, bool ELU>
 static int launch_agg_epi_nj(const GatAgg& p, const GatEpi& q0, cudaStream_t st) {
   int rc;
   GatEpi q = q0;
   q.n_main = (p.n_chunks + GAT_WARPS - 1) / GAT_WARPS;
   const int grid = p.n_seg + q.n_main;
   const size_t smem = (q.stat ? 2 * p.K : (p.n_seg > 0 ? p.K : 0)) * sizeof(float);
-  gat_aggregate_epi_kernel<V, NJ, U><<<grid, GAT_THREADS, smem, st>>>(p, q);
+  gat_aggregate_epi_kernel<V, NJ, U, ELU><<<grid, GAT_THREADS, smem, st>>>(p, q);
   if ((rc = check_launch())) return rc;
   if (p.n_hub > 0) {
-    gat_hub_finalize_epi_kernel<<<p.n_hub, GAT_THREADS, 0, st>>>(p.hub_rows, p.hub_segptr, p.ws, p.out, p.ldo, p.K, q);
+    gat_hub_finalize_epi_kernel<ELU><<<p.n_hub, GAT_THREADS, 0, st>>>(p.hub_rows, p.hub_segptr, p.ws, p.out, p.ldo, p.K, q);
     if ((rc = check_launch())) return rc;
   }
   return B200GNN_OK;
 }
-template <typename V>
+template <typename V, bool ELU = false>
 static int launch_agg_epi(const GatAgg& p, const GatEpi& q, cudaStream_t st) {   // the (NJ, U) choice of launch_agg
   constexpr int W = VecTraits<V>::W;
   const int nj = (p.K / W + 31) / 32;
   if constexpr (W == 4) {
-    if (nj <= 1) return launch_agg_epi_nj<V, 1, 8>(p, q, st);
-    if (nj <= 2) return launch_agg_epi_nj<V, 2, 4>(p, q, st);
+    if (nj <= 1) return launch_agg_epi_nj<V, 1, 8, ELU>(p, q, st);
+    if (nj <= 2) return launch_agg_epi_nj<V, 2, 4, ELU>(p, q, st);
   }
-  if (nj <= 4) return launch_agg_epi_nj<V, 4, 2>(p, q, st);
+  if (nj <= 4) return launch_agg_epi_nj<V, 4, 2, ELU>(p, q, st);
   if constexpr (W == 4) {
-    if (nj <= 8) return launch_agg_epi_nj<V, 8, 1>(p, q, st);
+    if (nj <= 8) return launch_agg_epi_nj<V, 8, 1, ELU>(p, q, st);
   }
-  return launch_agg_epi_nj<V, GAT_MAXJ, 1>(p, q, st);
+  return launch_agg_epi_nj<V, GAT_MAXJ, 1, ELU>(p, q, st);
 }
 
 template <typename V, int NJ, int U, bool SEG>
@@ -918,7 +928,7 @@ extern "C" int b200gnn_gat_aggregate_epi_f32(const int32_t* rowptr, const int32_
   p.H = (int32_t)H; p.D = (int32_t)D; p.K = (int32_t)K;
   GatEpi q;
   q.src_scale = src_scale; q.row_scale = row_scale; q.res = res; q.bias = bias; q.stat = stat_partial; q.ldr = res ? ldr : 0;
-  q.n_main = 0;
+  q.act = nullptr; q.lda = 0; q.n_main = 0;
   cudaStream_t st = (cudaStream_t)stream;
   const bool r4 = !res || (ldr % 4 == 0 && aligned_to(res, 16)), r2 = !res || (ldr % 2 == 0 && aligned_to(res, 8));
   const bool b4 = !bias || aligned_to(bias, 16), b2 = !bias || aligned_to(bias, 8);
@@ -970,5 +980,196 @@ extern "C" int b200gnn_gat_scores_bwd_f32(const float* ft, int64_t ldf, const fl
   if ((rc = check_launch())) return rc;
   gat_scores_bwd_finalize_kernel<<<(int)((2 * K + GAT_THREADS - 1) / GAT_THREADS), GAT_THREADS, 0, st>>>(
       partial, (int)used, (int)K, d_attn_l, attn_r ? d_attn_r : nullptr);
+  return check_launch();
+}
+
+// ---- the PyG GAT layers of the PPI models (engine_ppi.py): x = elu(GATConv(x) + Linear(x)) and the head-mean logits layer
+namespace b200gnn {
+
+// dZ = dA * (Z > 0 ? 1 : exp(Z)): torch's elu_backward (alpha 1, on the input), every operand with its own row pitch
+template <typename V>
+__global__ void __launch_bounds__(256) elu_bwd_kernel(const float* __restrict__ dA, int64_t ldda, const float* __restrict__ Z,
+                                                      int64_t ldz, float* __restrict__ dZ, int64_t lddz, int64_t n_rows, int kv) {
+  constexpr int W = VecTraits<V>::W;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n_rows * kv; i += (int64_t)gridDim.x * 256) {
+    const int64_t r = i / kv;
+    const int v = (int)(i - r * kv);
+    const V g = vldg(reinterpret_cast<const V*>(dA + (size_t)r * ldda) + v);
+    const V z = vldg(reinterpret_cast<const V*>(Z + (size_t)r * ldz) + v);
+    const float* gs = reinterpret_cast<const float*>(&g);
+    const float* zs = reinterpret_cast<const float*>(&z);
+    V o;
+    float* os = reinterpret_cast<float*>(&o);
+#pragma unroll
+    for (int w = 0; w < W; ++w) os[w] = zs[w] > 0.f ? gs[w] : gs[w] * expf(zs[w]);
+    reinterpret_cast<V*>(dZ + (size_t)r * lddz)[v] = o;
+  }
+}
+
+// Logits layer with concat=False (ppi_pyg/gnn.py:31,61 + the Linear skip) and its BCE / logit-KD loss (criterion.py:8-19).
+// One warp per row, lanes over the columns; per CTA the (classification, distillation) sums in fp64, warps added in order.
+constexpr int PPI_TAIL_MAX_SLOTS = 132 * 4;
+struct PpiTail {
+  const float* agg; const float* res; const float* b_conv; const float* b_lin; const float* y; const float* t;
+  float* logits; float* d_agg; float* d_res; double* partial;
+  int64_t lda, ldr, ldy, ldt, ldl, ldga, ldgr, n_rows;
+  int32_t H, Dp, C;
+  float w_cls, w_kd;            // d loss / d z = w_cls (sigmoid(z) - y) + w_kd (sigmoid(z) - sigmoid(t))
+};
+
+__global__ void __launch_bounds__(256) ppi_tail_kernel(const PpiTail p) {
+  __shared__ double s_red[8][2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double acc_c = 0.0, acc_k = 0.0;
+  const float hf = (float)p.H;
+  for (int64_t r = (int64_t)blockIdx.x * 8 + warp; r < p.n_rows; r += (int64_t)gridDim.x * 8) {
+    const float* ag = p.agg + (size_t)r * p.lda;
+    for (int c = lane; c < p.Dp; c += 32) {
+      if (c >= p.C) {                                      // padded columns of the gradients stay zero
+        if (p.y) {
+          for (int h = 0; h < p.H; ++h) p.d_agg[(size_t)r * p.ldga + h * p.Dp + c] = 0.f;
+          p.d_res[(size_t)r * p.ldgr + c] = 0.f;
+        }
+        continue;
+      }
+      float s = __ldg(ag + c);
+      for (int h = 1; h < p.H; ++h) s += __ldg(ag + h * p.Dp + c);
+      const float z = (s / hf + __ldg(p.b_conv + c)) + (__ldg(p.res + (size_t)r * p.ldr + c) + __ldg(p.b_lin + c));
+      p.logits[(size_t)r * p.ldl + c] = z;
+      if (!p.y) continue;
+      const float yv = __ldg(p.y + (size_t)r * p.ldy + c);
+      const float sp = log1pf(expf(-fabsf(z))), mz = fmaxf(z, 0.f);
+      const float sig = 1.f / (1.f + expf(-z));
+      acc_c += (double)(mz - z * yv + sp);
+      float dz = p.w_cls * (sig - yv);
+      if (p.t) {
+        const float tv = 1.f / (1.f + expf(-__ldg(p.t + (size_t)r * p.ldt + c)));
+        acc_k += (double)(mz - z * tv + sp);
+        dz += p.w_kd * (sig - tv);
+      }
+      p.d_res[(size_t)r * p.ldgr + c] = dz;
+      const float dh = dz / hf;                          // mean over heads: every head gets d z / H
+      for (int h = 0; h < p.H; ++h) p.d_agg[(size_t)r * p.ldga + h * p.Dp + c] = dh;
+    }
+  }
+  if (!p.y) return;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    acc_c += __shfl_xor_sync(FULL_MASK, acc_c, d);
+    acc_k += __shfl_xor_sync(FULL_MASK, acc_k, d);
+  }
+  if (lane == 0) { s_red[warp][0] = acc_c; s_red[warp][1] = acc_k; }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    double t = 0.0;
+    for (int w = 0; w < 8; ++w) t += s_red[w][threadIdx.x];
+    p.partial[(size_t)blockIdx.x * 2 + threadIdx.x] = t;
+  }
+}
+
+// loss_out = [alpha T^2 kd + (1 - alpha) cls, cls, kd] (KD) or [cls, cls, 0], the slots added in order
+__global__ void ppi_tail_finalize_kernel(const double* __restrict__ partial, int slots, double inv_n, int kd, float alpha, float T,
+                                         float* __restrict__ loss_out) {
+  double c = 0.0, k = 0.0;
+  for (int s = 0; s < slots; ++s) { c += partial[2 * s]; k += partial[2 * s + 1]; }
+  const float cls = (float)(c * inv_n), dis = (float)(k * inv_n);
+  loss_out[0] = kd ? dis * (alpha * T * T) + cls * (1.f - alpha) : cls;
+  loss_out[1] = cls;
+  loss_out[2] = kd ? dis : 0.f;
+}
+
+}  // namespace b200gnn
+
+extern "C" int b200gnn_gat_aggregate_elu_f32(const int32_t* rowptr, const int32_t* col, const int32_t* eidx, const float* a,
+                                             const float* ft, int64_t ldf, float* out, int64_t ldo, float* act, int64_t lda,
+                                             int64_t n_rows, int64_t H, int64_t D, const float* res, int64_t ldr,
+                                             const float* bias, const int32_t* chunk_rowptr, int64_t n_chunks,
+                                             int32_t hub_threshold, int32_t seg_len, const int32_t* hub_rows,
+                                             const int32_t* hub_segptr, int64_t n_hub, int64_t n_seg, float* hub_workspace,
+                                             void* stream) {
+  const int64_t K = H * D;
+  if (!rowptr || !a || !ft || !out || !act || n_rows < 0 || H <= 0 || D <= 0 || H > GAT_MAXH || ldf < K || ldo < K || lda < K ||
+      !chunk_rowptr || n_chunks < 0 || n_hub < 0 || n_seg < n_hub || (res && ldr < K) ||
+      (n_hub > 0 && (!hub_rows || !hub_segptr || !hub_workspace || seg_len <= 0)))
+    return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0 || n_chunks == 0) return B200GNN_OK;
+  GatAgg p;
+  p.rowptr = rowptr; p.col = col; p.eidx = eidx; p.chunk_rowptr = chunk_rowptr; p.hub_rows = hub_rows;
+  p.hub_segptr = hub_segptr; p.ws = hub_workspace;
+  p.a = a; p.ft = ft; p.out = out; p.ldf = ldf; p.ldo = ldo;
+  p.n_chunks = (int32_t)n_chunks; p.n_hub = (int32_t)n_hub; p.n_seg = (int32_t)(n_hub > 0 ? n_seg : 0); p.seg_len = seg_len;
+  p.hub_threshold = hub_threshold;
+  p.H = (int32_t)H; p.D = (int32_t)D; p.K = (int32_t)K;
+  GatEpi q;
+  q.src_scale = nullptr; q.row_scale = nullptr; q.res = res; q.bias = bias; q.stat = nullptr; q.ldr = res ? ldr : 0;
+  q.act = act; q.lda = lda; q.n_main = 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  // The vector width is chosen from the epi entry point's operands exactly as b200gnn_gat_aggregate_epi_f32 chooses it, so
+  // both run the same (V, NJ, U) instantiation shape and Z is its output bit for bit.  act must then take that width too
+  // (a narrower width would change U and with it the hub segments' summation order): otherwise the call is refused.
+  const bool r4 = !res || (ldr % 4 == 0 && aligned_to(res, 16)), r2 = !res || (ldr % 2 == 0 && aligned_to(res, 8));
+  const bool b4 = !bias || aligned_to(bias, 16), b2 = !bias || aligned_to(bias, 8);
+  if (D % 4 == 0 && ldf % 4 == 0 && ldo % 4 == 0 && aligned_to(ft, 16) && aligned_to(out, 16) && r4 && b4 &&
+      K <= 4 * 32 * GAT_MAXJ) {
+    if (lda % 4 || !aligned_to(act, 16)) return B200GNN_ERR_BAD_ARG;
+    return launch_agg_epi<float4, true>(p, q, st);
+  }
+  if (D % 2 == 0 && ldf % 2 == 0 && ldo % 2 == 0 && aligned_to(ft, 8) && aligned_to(out, 8) && r2 && b2 &&
+      K <= 2 * 32 * GAT_MAXJ) {
+    if (lda % 2 || !aligned_to(act, 8)) return B200GNN_ERR_BAD_ARG;
+    return launch_agg_epi<float2, true>(p, q, st);
+  }
+  if (K <= 32 * GAT_MAXJ) return launch_agg_epi<float, true>(p, q, st);
+  return B200GNN_ERR_UNSUPPORTED;
+}
+
+extern "C" int b200gnn_elu_bwd_f32(const float* dA, int64_t ldda, const float* Z, int64_t ldz, float* dZ, int64_t lddz,
+                                   int64_t n_rows, int64_t K, void* stream) {
+  if (!dA || !Z || !dZ || n_rows < 0 || K <= 0 || ldda < K || ldz < K || lddz < K) return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool v4 = K % 4 == 0 && ldda % 4 == 0 && ldz % 4 == 0 && lddz % 4 == 0 && aligned_to(dA, 16) && aligned_to(Z, 16) &&
+                  aligned_to(dZ, 16);
+  const int64_t kv = v4 ? K / 4 : K;
+  int64_t grid = (n_rows * kv + 255) / 256;
+  if (grid > 132 * 8) grid = 132 * 8;
+  if (v4) elu_bwd_kernel<float4><<<(int)grid, 256, 0, st>>>(dA, ldda, Z, ldz, dZ, lddz, n_rows, (int)kv);
+  else elu_bwd_kernel<float><<<(int)grid, 256, 0, st>>>(dA, ldda, Z, ldz, dZ, lddz, n_rows, (int)kv);
+  return check_launch();
+}
+
+extern "C" int64_t b200gnn_ppi_tail_slots(int64_t n_rows) {
+  if (n_rows < 0) return B200GNN_ERR_BAD_ARG;
+  const int64_t s = (n_rows + 7) / 8;
+  return s < 1 ? 1 : (s > PPI_TAIL_MAX_SLOTS ? PPI_TAIL_MAX_SLOTS : s);
+}
+
+extern "C" int b200gnn_ppi_logits_loss_f32(const float* agg, int64_t lda, const float* res, int64_t ldr, const float* b_conv,
+                                           const float* b_lin, int64_t n_rows, int64_t H, int64_t Dp, int64_t C,
+                                           float* logits, int64_t ldl, const float* labels, int64_t ldy,
+                                           const float* teacher_logits, int64_t ldt, float alpha, float T, float* d_agg,
+                                           int64_t ldga, float* d_res, int64_t ldgr, float* loss_out, double* partial,
+                                           int64_t slots, void* stream) {
+  if (!agg || !res || !b_conv || !b_lin || !logits || n_rows < 0 || H <= 0 || H > GAT_MAXH || C <= 0 || Dp < C ||
+      lda < H * Dp || ldr < C || ldl < C)
+    return B200GNN_ERR_BAD_ARG;
+  if (labels && (ldy < C || !d_agg || !d_res || !loss_out || !partial || ldga < H * Dp || ldgr < Dp ||
+                 slots < b200gnn_ppi_tail_slots(n_rows) || (teacher_logits && ldt < C) || n_rows == 0))
+    return B200GNN_ERR_BAD_ARG;
+  if (n_rows == 0) return B200GNN_OK;
+  PpiTail p;
+  p.agg = agg; p.res = res; p.b_conv = b_conv; p.b_lin = b_lin; p.y = labels; p.t = labels ? teacher_logits : nullptr;
+  p.logits = logits; p.d_agg = d_agg; p.d_res = d_res; p.partial = partial;
+  p.lda = lda; p.ldr = ldr; p.ldy = ldy; p.ldt = ldt; p.ldl = ldl; p.ldga = ldga; p.ldgr = ldgr; p.n_rows = n_rows;
+  p.H = (int32_t)H; p.Dp = (int32_t)Dp; p.C = (int32_t)C;
+  const double n_el = (double)n_rows * (double)C;
+  p.w_cls = (float)((p.t ? 1.0 - alpha : 1.0) / n_el);
+  p.w_kd = p.t ? (float)((double)alpha * T * T / n_el) : 0.f;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = (int)b200gnn_ppi_tail_slots(n_rows);
+  int rc;
+  ppi_tail_kernel<<<grid, 256, 0, st>>>(p);
+  if ((rc = check_launch()) || !labels) return rc;
+  ppi_tail_finalize_kernel<<<1, 1, 0, st>>>(partial, grid, 1.0 / n_el, p.t != nullptr, alpha, T, loss_out);
   return check_launch();
 }

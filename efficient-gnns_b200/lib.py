@@ -136,6 +136,13 @@ SIGNATURES = {
     "b200gnn_gat_aggregate_epi_f32": (_int, [_i32p, _i32p, _i32p, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64,
                                              _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _i64, _i32p, _i64, _i32, _i32,
                                              _i32p, _i32p, _i64, _i64, _f32p, _ptr]),
+    "b200gnn_gat_aggregate_elu_f32": (_int, [_i32p, _i32p, _i32p, _f32p, _f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64,
+                                             _i64, _f32p, _i64, _f32p, _i32p, _i64, _i32, _i32, _i32p, _i32p, _i64, _i64,
+                                             _f32p, _ptr]),
+    "b200gnn_elu_bwd_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _ptr]),
+    "b200gnn_ppi_tail_slots": (_i64, [_i64]),
+    "b200gnn_ppi_logits_loss_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _f32p, _i64, _i64, _i64, _i64, _f32p, _i64, _f32p,
+                                           _i64, _f32p, _i64, _f32, _f32, _f32p, _i64, _f32p, _i64, _f32p, _ptr, _i64, _ptr]),
     "b200gnn_graph_sort_workspace_bytes": (_i64, [_i64]),
     "b200gnn_graph_argsort_i64": (_int, [_ptr, _ptr, _i64, _i64, _i64, _i32p, _ptr, _ptr]),
     "b200gnn_graph_coalesce_i64": (_int, [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _i32p, _ptr, _ptr, _ptr, _ptr]),

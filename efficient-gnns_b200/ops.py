@@ -794,3 +794,70 @@ def gat_aggregate_epi(g: CsrGraph, eidx: Optional[torch.Tensor], a: torch.Tensor
         g.hub_rows.data_ptr() if g.n_hub else None, g.hub_segptr.data_ptr() if g.n_hub else None, g.n_hub, g.n_seg,
         None if ws is None else ws.data_ptr(), lib.stream_ptr()), "gat_aggregate_epi_f32")
     return out
+
+
+# ----------------------------------------------------------------------------- PPI GAT layers (engine_ppi.py)
+def gat_aggregate_elu(g: CsrGraph, a: torch.Tensor, ft: torch.Tensor, out: torch.Tensor, act: torch.Tensor, H: int,
+                      res: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """out = Z = Σ_e a[e,h]·ft[col[e],h,:] + res + bias (gat_aggregate_epi's output bit for bit) and act = elu(Z); ft / res / out /
+    act may be column blocks of wider matrices.  act must be aligned like out (same 16- or 8-byte vector width)."""
+    K = ft.shape[1]
+    fp, ldf = _rows(ft, "ft")
+    op, ldo = _rows(out, "out")
+    ap, lda = _rows(act, "act")
+    rp, ldr = _rows(res, "res") if res is not None else (None, 0)
+    ws = g.hub_workspace(K)
+    lib.check(lib.load().b200gnn_gat_aggregate_elu_f32(
+        g.rowptr.data_ptr(), g.col.data_ptr(), None, _f32(a, "a"), fp, ldf, op, ldo, ap, lda, g.n_rows, H, K // H, rp, ldr,
+        _f32(bias, "bias"), g.chunk_rowptr.data_ptr(), g.n_chunks, g.hub_threshold, g.seg_len,
+        g.hub_rows.data_ptr() if g.n_hub else None, g.hub_segptr.data_ptr() if g.n_hub else None, g.n_hub, g.n_seg,
+        None if ws is None else ws.data_ptr(), lib.stream_ptr()), "gat_aggregate_elu_f32")
+    return out, act
+
+
+def elu_bwd(d_act: torch.Tensor, z: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = d_act · (z > 0 ? 1 : exp(z)) (torch's elu_backward); every operand may be a column block (own row pitch)."""
+    n, K = z.shape
+    if d_act.shape != (n, K):
+        raise lib.B200GnnError("elu_bwd: d_act and z must have the same shape")
+    out = torch.empty(n, K, dtype=torch.float32, device=z.device) if out is None else out
+    gp, ldg = _rows(d_act, "d_act")
+    zp, ldz = _rows(z, "z")
+    op, ldo = _rows(out, "out")
+    lib.check(lib.load().b200gnn_elu_bwd_f32(gp, ldg, zp, ldz, op, ldo, n, K, lib.stream_ptr()), "elu_bwd_f32")
+    return out
+
+
+def ppi_tail_slots(n_rows: int) -> int:
+    return int(lib.load().b200gnn_ppi_tail_slots(n_rows))
+
+
+def ppi_logits_loss(agg: torch.Tensor, res: torch.Tensor, b_conv: torch.Tensor, b_lin: torch.Tensor, H: int, C: int,
+                    logits: torch.Tensor, labels: Optional[torch.Tensor] = None, teacher_logits: Optional[torch.Tensor] = None,
+                    alpha: float = 0.5, T: float = 1.0, d_agg: Optional[torch.Tensor] = None, d_res: Optional[torch.Tensor] = None,
+                    loss_out: Optional[torch.Tensor] = None, partial: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """logits[:, :C] = (mean_h agg + b_conv) + (res + b_lin) over agg [n, H·Dp] and res [n, >= Dp]; with labels also the BCE /
+    logit-KD loss into loss_out[3] and the seed gradients d_agg [n, H·Dp] (dz/H per head), d_res [n, >= Dp] (dz), padded
+    columns written as zero.  Every matrix may be a column block; partial: float64 [2·ppi_tail_slots(n)]."""
+    n = agg.shape[0]
+    Dp = agg.shape[1] // H
+    gp, lda = _rows(agg, "agg")
+    rp, ldr = _rows(res, "res")
+    lp, ldl = _rows(logits, "logits")
+    yp, ldy = _rows(labels, "labels") if labels is not None else (None, C)
+    tp, ldt = _rows(teacher_logits, "teacher_logits") if teacher_logits is not None else (None, C)
+    train = labels is not None
+    if train:
+        if d_agg is None or d_res is None or loss_out is None:
+            raise lib.B200GnnError("ppi_logits_loss: labels need d_agg, d_res and loss_out")
+        if partial is None:
+            partial = torch.empty(2 * ppi_tail_slots(n), dtype=torch.float64, device=agg.device)
+        if partial.dtype != torch.float64 or not partial.is_cuda or not partial.is_contiguous():
+            raise lib.B200GnnError("ppi_logits_loss: partial must be a contiguous CUDA float64 buffer")
+    dap, ldga = _rows(d_agg, "d_agg") if train else (None, H * Dp)
+    drp, ldgr = _rows(d_res, "d_res") if train else (None, Dp)
+    lib.check(lib.load().b200gnn_ppi_logits_loss_f32(
+        gp, lda, rp, ldr, _f32(b_conv, "b_conv"), _f32(b_lin, "b_lin"), n, H, Dp, C, lp, ldl, yp, ldy, tp, ldt, float(alpha),
+        float(T), dap, ldga, drp, ldgr, _f32(loss_out, "loss_out") if train else None,
+        partial.data_ptr() if train else None, partial.numel() // 2 if train else 0, lib.stream_ptr()), "ppi_logits_loss_f32")
+    return logits

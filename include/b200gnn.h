@@ -557,6 +557,42 @@ int b200gnn_gat_aggregate_epi_f32(const int32_t* rowptr, const int32_t* col, con
                                   int32_t seg_len, const int32_t* hub_rows, const int32_t* hub_segptr, int64_t n_hub,
                                   int64_t n_seg, float* hub_workspace, void* stream);
 
+/* ------------------------------------------------------------------ *
+ * The PyG GAT layers of the PPI models (engine_ppi.py; ppi_pyg/gnn.py:24-83): hidden layers x = elu(GATConv(x) + Linear(x)),
+ * a last layer GATConv(concat=False) + Linear.
+ *   gat_aggregate_elu : b200gnn_gat_aggregate_epi_f32 with res / bias (no scale vectors, no statistics) that also stores
+ *                       act = elu(out) (row pitch lda): out = Z is the epi entry point's output bit for bit (same plans,
+ *                       same vector width and summation order, hub rows through the same finalize), act is the next layer's
+ *                       GEMM operand.  act must admit the vector width the epi entry point picks for the other operands
+ *                       (16-byte base and lda % 4 == 0 when out / ft / res / bias do; 8-byte and even lda for the float2
+ *                       path), else B200GNN_ERR_BAD_ARG.
+ *   elu_bwd           : dZ = dA * (Z > 0 ? 1 : exp(Z)) (torch's elu_backward), every operand with its own row pitch.
+ *   ppi_logits_loss   : logits[r, c] = (mean_h agg[r, h*Dp + c] + b_conv[c]) + (res[r, c] + b_lin[c]) for c < C (agg [n, H*Dp]
+ *                       from the plain aggregation, res [n, >= Dp]).  With labels (float multi-hot, [n, C] pitch ldy) also
+ *                       the loss over all n*C entries: BCE-with-logits, or with teacher logits the logit KD alpha T^2
+ *                       BCE(z, sigmoid(t)) + (1 - alpha) BCE(z, y); loss_out[3] = [loss, loss_cls, loss_kd] ([cls, cls, 0]
+ *                       without a teacher); d_agg[r, h*Dp + c] = dz / H in every head, d_res[r, c] = dz, columns C..Dp-1
+ *                       of both written as zero.  Per-CTA fp64 sums in partial (double[2 * slots], slots >=
+ *                       b200gnn_ppi_tail_slots(n)), added in slot order: no atomics, repeatable.  Without labels only the
+ *                       logits are written (eval).
+ * ------------------------------------------------------------------ */
+int b200gnn_gat_aggregate_elu_f32(const int32_t* rowptr, const int32_t* col, const int32_t* eidx, const float* a,
+                                  const float* ft, int64_t ldf, float* out, int64_t ldo, float* act, int64_t lda,
+                                  int64_t n_rows, int64_t H, int64_t D, const float* res, int64_t ldr,
+                                  const float* bias, const int32_t* chunk_rowptr, int64_t n_chunks,
+                                  int32_t hub_threshold, int32_t seg_len, const int32_t* hub_rows,
+                                  const int32_t* hub_segptr, int64_t n_hub, int64_t n_seg, float* hub_workspace,
+                                  void* stream);
+int b200gnn_elu_bwd_f32(const float* dA, int64_t ldda, const float* Z, int64_t ldz, float* dZ, int64_t lddz,
+                        int64_t n_rows, int64_t K, void* stream);
+int64_t b200gnn_ppi_tail_slots(int64_t n_rows);
+int b200gnn_ppi_logits_loss_f32(const float* agg, int64_t lda, const float* res, int64_t ldr, const float* b_conv,
+                                const float* b_lin, int64_t n_rows, int64_t H, int64_t Dp, int64_t C,
+                                float* logits, int64_t ldl, const float* labels, int64_t ldy,
+                                const float* teacher_logits, int64_t ldt, float alpha, float T, float* d_agg,
+                                int64_t ldga, float* d_res, int64_t ldgr, float* loss_out, double* partial,
+                                int64_t slots, void* stream);
+
 /* ------------------------------------------------------------------
  * Peer-memory exchange of the node-parallel engine (SURVEY.md §8e; no reference counterpart: the reference is
  * single-GPU, arxiv_pyg/scripts/run_gcn.sh:24-28).  One process per GPU; each rank allocates an exchange arena,
