@@ -458,6 +458,26 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
 }
 __global__ void adam_tick_kernel(int32_t* step) { *step += 1; }
 
+// ---------------------------------------------------------------- RMSprop (torch.optim.RMSprop: no momentum, not centred)
+// The operations of torch's single-tensor CPU update, each rounded on its own (no contraction):
+//   g = grad + wd * p;  sq = sq * alpha + (1 - alpha) * g * g;  p = p + (-lr_t * g) / (sqrt(sq) + eps)
+// lr_t = lr * min(step + 1, warmup) / warmup formed in double and rounded once (adjust_learning_rate, arxiv_dgl/gat.py:110-113);
+// warmup <= 0: lr_t = lr.
+__global__ void __launch_bounds__(256) rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq,
+                                                      int64_t n, double lr, int warmup, float alpha, float one_minus_alpha,
+                                                      float eps, float wd, const int32_t* __restrict__ step) {
+  const int e = *step + 1;
+  const float neg_lr = -(float)(warmup > 0 ? lr * (double)(e < warmup ? e : warmup) / (double)warmup : lr);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float pi = p[i];
+    float gi = g[i];
+    if (wd != 0.f) gi = __fadd_rn(gi, __fmul_rn(wd, pi));
+    const float s = __fadd_rn(__fmul_rn(sq[i], alpha), __fmul_rn(__fmul_rn(one_minus_alpha, gi), gi));
+    sq[i] = s;
+    p[i] = __fadd_rn(pi, __fdiv_rn(__fmul_rn(neg_lr, gi), __fadd_rn(__fsqrt_rn(s), eps)));
+  }
+}
+
 static inline int grid_for(int64_t n_items, int per_cta, int cap = 132 * 8) {
   int64_t g = (n_items + per_cta - 1) / per_cta;
   if (g > cap) g = cap;
@@ -723,6 +743,23 @@ extern "C" int b200gnn_adam_step_f32(float* params, const float* grads, float* e
   int rc;
   if (n > 0) {
     adam_kernel<<<grid_for(n, 256), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, step);
+    if ((rc = check_launch())) return rc;
+  }
+  adam_tick_kernel<<<1, 1, 0, st>>>(step);
+  return check_launch();
+}
+
+extern "C" int b200gnn_rmsprop_step_f32(float* params, const float* grads, float* square_avg, int64_t n, double lr,
+                                        int64_t warmup, double alpha, double eps, double weight_decay, int32_t* step,
+                                        void* stream) {
+  if (!params || !grads || !square_avg || !step || n < 0 || !(lr >= 0.0) || !(alpha >= 0.0) || !(eps >= 0.0) ||
+      !(weight_decay >= 0.0) || warmup < 0 || warmup > (1 << 30))
+    return B200GNN_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (n > 0) {
+    rmsprop_kernel<<<grid_for(n, 256), 256, 0, st>>>(params, grads, square_avg, n, lr, (int)warmup, (float)alpha,
+                                                     (float)(1.0 - alpha), (float)eps, (float)weight_decay, step);
     if ((rc = check_launch())) return rc;
   }
   adam_tick_kernel<<<1, 1, 0, st>>>(step);

@@ -49,7 +49,10 @@ class GATTrainer:
     def __init__(self, adj: SparseTensor, in_feats: int, n_classes: int, n_hidden: int, n_layers: int, n_heads: int,
                  dropout: float = 0.0, input_drop: float = 0.0, edge_drop: float = 0.0, use_attn_dst: bool = True,
                  use_symmetric_norm: bool = False, lr: float = 0.002, seed: int = 0, alpha: float = 0.9, T: float = 4.0,
-                 attn_drop: float = 0.0, negative_slope: float = 0.2, bn_eps: float = 1e-5, bn_momentum: float = 0.1):
+                 attn_drop: float = 0.0, negative_slope: float = 0.2, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
+                 step_streams: Optional[int] = None):
+        """step_streams: Philox offsets one training step spans (default 2 * n_layers, one forward's streams); a recipe that
+        runs several training forwards per step passes more and draws forward f at stream base f * 2 * n_layers."""
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         if attn_drop != 0.0:
             raise ValueError("attn_drop > 0 is not implemented (every reference configuration passes 0)")
@@ -68,6 +71,7 @@ class GATTrainer:
         self.lr, self.seed, self.alpha, self.kd_T = float(lr), int(seed), float(alpha), float(T)
         self.slope, self.bn_eps, self.bn_momentum = float(negative_slope), bn_eps, bn_momentum
         N, L = self.N, self.L
+        self.step_mul = 2 * L if step_streams is None else int(step_streams)
 
         self.G = st.engine_csr_unweighted() if st.value() is None else st.engine_csr()
         self.Gt = st.engine_csc("value")
@@ -268,21 +272,24 @@ class GATTrainer:
         self._load_vec(self.bias_last, self.L - 1, sd["bias_last.bias"])
 
     # ------------------------------------------------------------------ forward
-    def stream_offset(self, kind: str, layer: int, step: int) -> int:
-        """Philox offset of a random stream of training step ``step``: 'dropout' (hidden layer), 'input', 'edge' (layer)."""
+    def stream_offset(self, kind: str, layer: int, step: int, fwd: int = 0) -> int:
+        """Philox offset of a random stream of training forward ``fwd`` of step ``step``: 'dropout' (hidden layer), 'input',
+        'edge' (layer)."""
         base = {"dropout": layer, "input": self.L - 1, "edge": self.L + layer}[kind]
-        return base + step * 2 * self.L
+        return base + fwd * 2 * self.L + step * self.step_mul
 
-    def _draw(self):
-        """All keep decisions of the step: they need no input, so they run on the side stream next to the first GEMM."""
-        mul = 2 * self.L
+    def _draw(self, base: int = 0):
+        """All keep decisions of the step: they need no input, so they run on the side stream next to the first GEMM.
+        base: the first Philox offset of this forward's streams within the step."""
+        mul = self.step_mul
         if self.p > 0:
-            ops.dropout_bits(self.keep_bits, self.p, self.seed, 0, step_dev=self.step_count, step_mul=mul)
+            ops.dropout_bits(self.keep_bits, self.p, self.seed, base, step_dev=self.step_count, step_mul=mul)
         if self.p_in > 0:
-            ops.dropout_bits(self.in_bits, self.p_in, self.seed, self.L - 1, step_dev=self.step_count, step_mul=mul, K=self.in_feats)
+            ops.dropout_bits(self.in_bits, self.p_in, self.seed, base + self.L - 1, step_dev=self.step_count, step_mul=mul,
+                             K=self.in_feats)
         if self.p_edge > 0:
             for l in range(self.L):
-                ops.dropout_mask_step(self.edge_keep[l], self.p_edge, self.seed, self.L + l, self.step_count, mul)
+                ops.dropout_mask_step(self.edge_keep[l], self.p_edge, self.seed, base + self.L + l, self.step_count, mul)
 
     def _act(self, l: int):
         """(Y, scale, shift, keep bits, p) from which the fused kernels form hidden activation l of the last forward."""
@@ -290,8 +297,8 @@ class GATTrainer:
             return self.Y[l], self.bn[l][2], self.bn[l][3], self.keep_bits[l], self.p
         return self.Y[l], self.bn_eval[l][0], self.bn_eval[l][1], self.ones_bits, 0.0
 
-    def forward(self, x: torch.Tensor, training: bool = True) -> torch.Tensor:
-        """Logits [N, n_classes]; training=False uses the running statistics and draws nothing."""
+    def forward(self, x: torch.Tensor, training: bool = True, stream_base: int = 0) -> torch.Tensor:
+        """Logits [N, n_classes]; training=False uses the running statistics and draws nothing.  stream_base: see _draw."""
         self._training = training
         L_ = lib.load()
         draws = training and (self.p > 0 or self.p_in > 0 or self.p_edge > 0)
@@ -299,7 +306,7 @@ class GATTrainer:
             self._ev_fork.record(torch.cuda.current_stream())
             self._side.wait_event(self._ev_fork)
             with torch.cuda.stream(self._side):
-                self._draw()
+                self._draw(stream_base)
                 self._ev_bits.record(self._side)
         for l in range(self.L):
             H, K, last = self.Hl[l], self.K[l], l == self.L - 1

@@ -25,6 +25,7 @@ _i64 = C.c_int64
 _i32 = C.c_int32
 _int = C.c_int
 _f32 = C.c_float
+_f64 = C.c_double
 _u64 = C.c_uint64
 
 # name -> (restype, argtypes).  tests/test_abi.py checks this table against the header.
@@ -67,6 +68,15 @@ SIGNATURES = {
                                             _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _ptr]),
     "b200gnn_partial_reduce_f32": (_int, [_f32p, _i64, _i64, _f32p, _ptr]),
     "b200gnn_adam_step_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _f32, _f32, _f32, _f32, _i32p, _ptr]),
+    "b200gnn_rmsprop_step_f32": (_int, [_f32p, _f32p, _f32p, _i64, _f64, _i64, _f64, _f64, _f64, _i32p, _ptr]),
+    "b200gnn_teacher_slots": (_i64, [_i64]),
+    "b200gnn_label_inputs_f32": (_int, [_f32p, _i64, _i64, _i64, _i64, _i32p, _ptr, _int, _f32, _u64, _u64, _i32p, _u64, _ptr,
+                                        _int, _ptr, _i32p, _ptr]),
+    "b200gnn_label_softmax_f32": (_int, [_f32p, _i64, _i64, _i64, _ptr, _int, _f32p, _i64, _ptr]),
+    "b200gnn_logce_fwd_bwd_f32": (_int, [_f32p, _i64, _i64, _ptr, _i64, _ptr, _ptr, _i32p, _i64, _f32p, _i64, _f32p, _f32p,
+                                         _ptr, _ptr]),
+    "b200gnn_split_eval_f32": (_int, [_f32p, _i64, _i64, _ptr, _i64, _i64, _i64, _ptr, _f32p, _f32p, _ptr, _ptr]),
+    "b200gnn_snapshot_if_better_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _i64, _f32p, _f32p, _i64, _ptr]),
     "b200gnn_kd_partials": (_i64, [_i64]),
     "b200gnn_kd_loss_fwd_bwd_f32": (_int, [_f32p, _i64, _ptr, _i64, _ptr, _f32p, _i64, _i64, _f32, _f32, _i64, _f32p,
                                            _i64, _f32p, _f32p, _ptr]),

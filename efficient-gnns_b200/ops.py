@@ -861,3 +861,90 @@ def ppi_logits_loss(agg: torch.Tensor, res: torch.Tensor, b_conv: torch.Tensor, 
         float(T), dap, ldga, drp, ldgr, _f32(loss_out, "loss_out") if train else None,
         partial.data_ptr() if train else None, partial.numel() // 2 if train else 0, lib.stream_ptr()), "ppi_logits_loss_f32")
     return logits
+
+
+# ---------------------------------------------------------------------------------------------- GAT teacher recipe
+ROLE_NONE, ROLE_INPUT, ROLE_PRED, ROLE_EVAL = 0, 1, 2, 3
+
+
+def rmsprop_step(params, grads, square_avg, step: torch.Tensor, lr: float, warmup: int = 0, alpha: float = 0.99,
+                 eps: float = 1e-8, weight_decay: float = 0.0):
+    """torch.optim.RMSprop (no momentum, not centred) over flat buffers; the rate is lr * min(step + 1, warmup) / warmup
+    (warmup 0: lr) with the step read on the device, which is then incremented."""
+    lib.check(lib.load().b200gnn_rmsprop_step_f32(
+        _f32(params, "params"), _f32(grads, "grads"), _f32(square_avg, "square_avg"), params.numel(), float(lr), int(warmup),
+        float(alpha), float(eps), float(weight_decay), lib.dptr(step, torch.int32, "step"), lib.stream_ptr()), "rmsprop_step_f32")
+
+
+def teacher_slots(n_items: int) -> int:
+    return int(lib.load().b200gnn_teacher_slots(n_items))
+
+
+def label_inputs(X: Optional[torch.Tensor], col0: int, C: int, row_pos: torch.Tensor, labels: Optional[torch.Tensor],
+                 role: torch.Tensor, cnt_part: torch.Tensor, eval: bool, use_labels: bool, mask_rate: float = 0.0,
+                 seed: int = 0, offset: int = 0, step_dev: Optional[torch.Tensor] = None, step_mul: int = 0,
+                 mask: Optional[torch.Tensor] = None):
+    """Roles of every row and (use_labels) the label block X[:, col0:col0+C]: one-hot for the label rows, zero elsewhere;
+    cnt_part[teacher_slots(N)] receives the per-CTA counts of loss rows.  mask (uint8 [n_train]) replaces the Philox
+    label mask."""
+    n = row_pos.numel()
+    if role.dtype != torch.uint8 or role.numel() != n or cnt_part.dtype != torch.int32 or cnt_part.numel() != teacher_slots(n):
+        raise lib.B200GnnError("label_inputs: role must be uint8[N] and cnt_part int32[teacher_slots(N)]")
+    xp, ldx = _rows(X, "X") if C > 0 else (None, 0)
+    lib.check(lib.load().b200gnn_label_inputs_f32(
+        xp, ldx, col0, C if use_labels else 0, n, lib.dptr(row_pos, torch.int32, "row_pos"),
+        lib.dptr(labels, torch.int64, "labels"), int(eval), float(mask_rate), seed, offset,
+        lib.dptr(step_dev, torch.int32, "step_dev"), step_mul, lib.dptr(mask, torch.uint8, "mask"), int(use_labels),
+        role.data_ptr(), cnt_part.data_ptr(),
+        lib.stream_ptr()), "label_inputs_f32")
+
+
+def label_softmax(logits: torch.Tensor, C: int, out: torch.Tensor, role: Optional[torch.Tensor] = None, role_mask: int = 0):
+    """out[r, :C] = softmax(logits[r, :C]) for the rows whose role bit is in role_mask (all rows without roles)."""
+    lp, ld = _rows(logits, "logits")
+    op, ldo = _rows(out, "out")
+    if role is not None and (role.dtype != torch.uint8 or role.numel() != logits.shape[0]):
+        raise lib.B200GnnError("label_softmax: role must be uint8[N]")
+    lib.check(lib.load().b200gnn_label_softmax_f32(lp, ld, C, logits.shape[0], None if role is None else role.data_ptr(),
+                                                   int(role_mask), op, ldo, lib.stream_ptr()), "label_softmax_f32")
+    return out
+
+
+def logce_fwd_bwd(logits: torch.Tensor, C: int, train_idx: torch.Tensor, labels: torch.Tensor, role: torch.Tensor,
+                  cnt_part: torch.Tensor, d_logits: torch.Tensor, loss_out: torch.Tensor, acc_out: torch.Tensor,
+                  partial: torch.Tensor):
+    """The log-CE loss of the role-2 rows (device-counted) with its gradient into d_logits, and the training accuracy."""
+    lp, ld = _rows(logits, "logits")
+    dp, ldd = _rows(d_logits, "d_logits")
+    if partial.dtype != torch.float64 or partial.numel() < 6 * teacher_slots(train_idx.numel()):
+        raise lib.B200GnnError("logce: partial must be float64[6 * teacher_slots(n_train)]")
+    lib.check(lib.load().b200gnn_logce_fwd_bwd_f32(
+        lp, ld, C, lib.dptr(train_idx, torch.int64, "train_idx"), train_idx.numel(), lib.dptr(labels, torch.int64, "labels"),
+        role.data_ptr(), lib.dptr(cnt_part, torch.int32, "cnt_part"), cnt_part.numel(), dp, ldd, loss_out.data_ptr(),
+        acc_out.data_ptr(), partial.data_ptr(), lib.stream_ptr()), "logce_fwd_bwd_f32")
+
+
+def split_eval(logits: torch.Tensor, C: int, idx: torch.Tensor, sizes, labels: torch.Tensor, loss_out: torch.Tensor,
+               acc_out: torch.Tensor, partial: torch.Tensor):
+    """Log-CE loss and first-maximum accuracy of the three splits of idx = [train | val | test] (sizes n0, n1, n2)."""
+    lp, ld = _rows(logits, "logits")
+    n0, n1, n2 = (int(s) for s in sizes)
+    if partial.dtype != torch.float64 or partial.numel() < 6 * teacher_slots(n0 + n1 + n2) or idx.numel() != n0 + n1 + n2:
+        raise lib.B200GnnError("split_eval: partial must be float64[6 * teacher_slots(len(idx))]")
+    lib.check(lib.load().b200gnn_split_eval_f32(lp, ld, C, lib.dptr(idx, torch.int64, "idx"), n0, n1, n2,
+                                                lib.dptr(labels, torch.int64, "labels"), loss_out.data_ptr(), acc_out.data_ptr(),
+                                                partial.data_ptr(), lib.stream_ptr()), "split_eval_f32")
+
+
+def snapshot_if_better(cand: torch.Tensor, best: torch.Tensor, pairs):
+    """If cand < best (a NaN never is): copy every (src, dst) pair of contiguous fp32 buffers, then best = cand."""
+    args = []
+    for s, d in list(pairs) + [(None, None)] * (3 - len(pairs)):
+        if s is None:
+            args += [None, None, 0]
+        else:
+            if s.numel() != d.numel():
+                raise lib.B200GnnError("snapshot: source and destination sizes differ")
+            args += [_f32(s, "src"), _f32(d, "dst"), s.numel()]
+    lib.check(lib.load().b200gnn_snapshot_if_better_f32(cand.data_ptr(), best.data_ptr(), *args, lib.stream_ptr()),
+              "snapshot_if_better_f32")

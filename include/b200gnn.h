@@ -244,6 +244,50 @@ int b200gnn_partial_reduce_f32(const float* partial, int64_t slots, int64_t K2,
 int b200gnn_adam_step_f32(float* params, const float* grads, float* exp_avg,
                           float* exp_avg_sq, int64_t n, float lr, float beta1,
                           float beta2, float eps, int32_t* step, void* stream);
+/* torch.optim.RMSprop(lr, alpha, eps, weight_decay) without momentum or centring over flat buffers, with the linear warm-up
+ * of arxiv_dgl/gat.py:110-113: the rate of the step is lr * min(*step + 1, warmup) / warmup, formed in double and rounded
+ * once (warmup = 0: lr).  *step (device int32, steps already taken) is incremented.  An entry with zero parameter and
+ * gradient keeps zero parameter and square_avg. */
+int b200gnn_rmsprop_step_f32(float* params, const float* grads, float* square_avg, int64_t n, double lr, int64_t warmup,
+                             double alpha, double eps, double weight_decay, int32_t* step, void* stream);
+
+/* ------------------------------------------------------------------ *
+ * The training recipe of the arxiv GAT teacher (arxiv_dgl/gat.py:98-183).  Every call is graph-capturable: the step
+ * counter, the loss-row count and the best loss are read on the device.
+ * role (uint8[n_rows]): 0 none, 1 input (a training row whose label is an input, or without labels a training row outside
+ * the loss), 2 pred (a training row the loss runs on), 3 val / test.
+ * cnt_part: int32[b200gnn_teacher_slots(n_rows)], the per-CTA count of role-2 rows.
+ * partial: double[6 * b200gnn_teacher_slots(rows visited)] scratch.  C <= 256.
+ * ------------------------------------------------------------------ */
+int64_t b200gnn_teacher_slots(int64_t n_items);
+/* Roles and the label block X[:, col0 : col0 + C] of every row: one-hot labels[r] for role-1 rows when C > 0, zero for
+ * every other row.  row_pos[r]: position in train_idx (>= 0), -1 for val / test, -2 otherwise.  Training (eval == 0):
+ * training position j is masked iff b200gnn_dropout_mask_u8 at p = mask_rate drops flat element j for the offset
+ * offset + *step_dev * step_mul; masked rows are the label rows (use_labels) or the loss rows (no labels).  eval != 0:
+ * every training row is a label row and nothing is drawn (step_dev may be NULL).  mask_in (uint8[n_train], optional)
+ * replaces the draw with a given mask, e.g. a recorded torch.rand draw. */
+int b200gnn_label_inputs_f32(float* X, int64_t ldx, int64_t col0, int64_t C, int64_t n_rows, const int32_t* row_pos,
+                             const int64_t* labels, int eval, float mask_rate, uint64_t seed, uint64_t offset,
+                             const int32_t* step_dev, uint64_t step_mul, const uint8_t* mask_in, int use_labels, uint8_t* role,
+                             int32_t* cnt_part, void* stream);
+/* out[r, 0:C] = softmax(logits[r, 0:C]) for every row with bit role[r] set in role_mask (every row when role is NULL). */
+int b200gnn_label_softmax_f32(const float* logits, int64_t ld, int64_t C, int64_t n_rows, const uint8_t* role, int role_mask,
+                              float* out, int64_t ldo, void* stream);
+/* custom_loss_function (gat.py:98-101) over the role-2 rows of train_idx: loss_out[0] = mean(log(eps + CE_i) - log eps),
+ * eps = 1 - ln 2, normalised by the device count of role-2 rows; dlogits of those rows = (softmax - onehot) /
+ * ((eps + CE_i) * n) (the caller zeroes the rest); acc_out[0] = first-maximum argmax accuracy over all of train_idx. */
+int b200gnn_logce_fwd_bwd_f32(const float* logits, int64_t ld, int64_t C, const int64_t* train_idx, int64_t n_train,
+                              const int64_t* labels, const uint8_t* role, const int32_t* cnt_part, int64_t n_cnt,
+                              float* dlogits, int64_t ldd, float* loss_out, float* acc_out, double* partial, void* stream);
+/* evaluate()'s losses and accuracies (gat.py:168-183): idx = [train | val | test] (sizes n0, n1, n2);
+ * loss_out[s] = custom_loss_function, acc_out[s] = first-maximum argmax accuracy of split s. */
+int b200gnn_split_eval_f32(const float* logits, int64_t ld, int64_t C, const int64_t* idx, int64_t n0, int64_t n1, int64_t n2,
+                           const int64_t* labels, float* loss_out, float* acc_out, double* partial, void* stream);
+/* The best-epoch snapshot (gat.py:217-222): if *cand < *best (never for NaN), dst_i = src_i (n_i floats, a multiple of 4,
+ * 16-byte aligned; n_i = 0 skips), then *best = *cand. */
+int b200gnn_snapshot_if_better_f32(const float* cand, float* best, const float* src0, float* dst0, int64_t n0,
+                                   const float* src1, float* dst1, int64_t n1, const float* src2, float* dst2, int64_t n2,
+                                   void* stream);
 
 /* ------------------------------------------------------------------ *
  * Row-wise classification / logit-KD loss with its gradient in one pass.
