@@ -667,6 +667,9 @@ extern "C" int b200gnn_bn_act_bwd_reduce_f32(const float* dOut, const float* Xou
   if (!rows_ok(n_rows, K) || n_rows == 0 || !dOut || !Xout || !Y || !mean || !invstd || !partial || slots < 1 ||
       p < 0.f || p >= 1.f)
     return B200GNN_ERR_BAD_ARG;
+  // every operand is read as float4
+  if (!aligned_to(dOut, 16) || !aligned_to(Xout, 16) || !aligned_to(Y, 16) || !aligned_to(mean, 16) || !aligned_to(invstd, 16))
+    return B200GNN_ERR_BAD_ARG;
   if (ROWS_THREADS / (K / 4) < 1) return B200GNN_ERR_UNSUPPORTED;
   const float inv_keep = p > 0.f ? 1.f / (1.f - p) : 1.f;
   bn_act_bwd_reduce_kernel<<<(int)slots, ROWS_THREADS, 2 * K * sizeof(float), (cudaStream_t)stream>>>(
@@ -685,6 +688,10 @@ extern "C" int b200gnn_bn_act_bwd_apply_f32(const float* dOut, const float* Xout
                                             int64_t slots, float* coef, void* stream) {
   if (!rows_ok(n_rows, K) || n_rows == 0 || !dOut || !Y || !mean || !invstd || !gamma || !sums || !dY ||
       !dgamma || !dbeta || !partial || !coef || slots < 1 || sum_slots < 1 || n_norm < 1 || p < 0.f || p >= 1.f)
+    return B200GNN_ERR_BAD_ARG;
+  // the apply pass reads dOut, Xout, Y, mean, invstd and coef and writes dY as float4
+  if (!aligned_to(dOut, 16) || (Xout && !aligned_to(Xout, 16)) || !aligned_to(Y, 16) || !aligned_to(mean, 16) ||
+      !aligned_to(invstd, 16) || !aligned_to(coef, 16) || !aligned_to(dY, 16))
     return B200GNN_ERR_BAD_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const float inv_keep = p > 0.f ? 1.f / (1.f - p) : 1.f;

@@ -11,27 +11,6 @@ from oracle import criterion as oc
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("n,K", [(2, 4), (257, 40), (5000, 64), (3001, 256), (777, 1024)])
-def test_col_stats_and_bn_finalize(n, K):
-    g = torch.Generator().manual_seed(n + K)
-    y = torch.randn(n, K, generator=g) * 3 + 1.5
-    gamma, beta = torch.rand(K, generator=g) + 0.5, torch.randn(K, generator=g)
-    rm, rv = torch.zeros(K), torch.ones(K)
-    part = ops.col_stats(y.cuda())
-    out = ops.bn_finalize(part, n, gamma.cuda(), beta.cuda(), 1e-5, 0.1, rmc := rm.cuda(), rvc := rv.cuda()).cpu()
-    yd = y.double()
-    mean, var = yd.mean(0), yd.var(0, unbiased=False)
-    assert rel_err(out[0], mean) < 1e-5
-    assert rel_err(out[1], 1 / torch.sqrt(var + 1e-5)) < 1e-5
-    bn = torch.nn.BatchNorm1d(K).double()
-    if n > 1:
-        bn.train(); bn(yd)
-        assert rel_err(rmc, bn.running_mean) < 1e-5 and rel_err(rvc, bn.running_var) < 1e-5
-    z = ops.affine_relu_dropout(y.cuda(), out[2].cuda(), out[3].cuda(), relu=False, p=0.0)
-    ref = (yd - mean) / torch.sqrt(var + 1e-5) * gamma.double() + beta.double()
-    assert rel_err(z, ref) < 1e-5
-
-
 def test_dropout_mask_is_replayable_and_unbiased():
     n, K, p = 4000, 256, 0.5
     y = torch.ones(n, K, device="cuda")
@@ -45,29 +24,6 @@ def test_dropout_mask_is_replayable_and_unbiased():
     assert abs(float(m.float().mean()) - 0.5) < 5e-3
     # columns/rows are not correlated with the element index pattern
     assert float(m.float().mean(0).std()) < 0.02 and float(m.float().mean(1).std()) < 0.06
-
-
-@pytest.mark.parametrize("n,K,p", [(2000, 64, 0.0), (3001, 256, 0.5), (500, 40, 0.3)])
-def test_bn_relu_dropout_backward_matches_autograd(n, K, p):
-    g = torch.Generator().manual_seed(K)
-    y = torch.randn(n, K, generator=g) * 2 + 0.3
-    gamma, beta = torch.rand(K, generator=g) + 0.5, torch.randn(K, generator=g) * 0.1
-    d_out = torch.randn(n, K, generator=g)
-    yc = y.cuda()
-    bn = ops.bn_finalize(ops.col_stats(yc), n, gamma.cuda(), beta.cuda())
-    x_out = ops.affine_relu_dropout(yc, bn[2], bn[3], True, p, seed=1, offset=0)
-    mask = ops.dropout_mask(n, K, p, 1, 0).cpu().double() if p > 0 else torch.ones(n, K, dtype=torch.double)
-    d_y, d_gamma, d_beta, d_bias = ops.bn_act_bwd(d_out.cuda(), x_out, yc, bn[0], bn[1], gamma.cuda(), p)
-    # fp64 autograd reference
-    yr = y.double().requires_grad_(True)
-    gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
-    z = (yr - yr.mean(0)) / torch.sqrt(yr.var(0, unbiased=False) + 1e-5) * gr + br
-    out = torch.relu(z) * mask / (1 - p)
-    assert rel_err(x_out, out) < 1e-5
-    out.backward(d_out.double())
-    assert rel_err(d_y, yr.grad) < 2e-5
-    assert rel_err(d_gamma, gr.grad) < 2e-5 and rel_err(d_beta, br.grad) < 2e-5
-    assert d_bias.abs().max().item() < 1e-4 * yr.grad.abs().sum(0).max().item()   # sum_rows dY == 0 analytically
 
 
 def test_col_sum():
