@@ -398,6 +398,57 @@ def lpw_criterion(logits, labels, feat, teacher_feat, edge_index, kernel='cosine
 NCE_CHUNK_BYTES = 32 << 20
 
 
+def nce_chunk_rows(Sp: int) -> int:
+    """Rows R of one [R, Sp] logits chunk (R * Sp * 4 <= NCE_CHUNK_BYTES, a multiple of 128, at most Sp)."""
+    return min(max(128, (NCE_CHUNK_BYTES // (4 * Sp)) // 128 * 128), Sp)
+
+
+class NceBuffers:
+    """Every buffer of one InfoNCE forward + gradient over [Sp, Fp] operands: allocated once, so that a captured step (gcrd.py)
+    reuses them on every replay.  g_s / g_t (d loss / d xs, d xt, [Sp, Fp]) exist when requested."""
+
+    def __init__(self, Sp: int, Fp: int, device, need_s: bool = True, need_t: bool = True):
+        R = nce_chunk_rows(Sp)
+        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=device)
+        self.Z, self.part, self.loss = e(R, Sp), e(Sp), e(1)
+        self.xt_split = (e(Sp, Fp), e(Sp, Fp))                                    # B of Z_c = xs_c · xt^T
+        self.g_s = e(Sp, Fp) if need_s else None
+        self.xtT_split = (e(Fp, Sp), e(Fp, Sp)) if need_s else None                # B of dZ_c · xt
+        self.g_t = e(Sp, Fp) if need_t else None
+        self.Zt = e(Sp * R) if need_t else None
+        self.xsT_split = (e(Fp * R), e(Fp * R)) if need_t else None                # B of dZ_c^T · xs_c, per chunk
+
+
+def nce_chunks(xs_p: torch.Tensor, xt_p: torch.Tensor, S: int, b: NceBuffers) -> None:
+    """The chunk loop of the G-CRD loss over zero-padded operands xs_p, xt_p [Sp, Fp] (S real rows; xs_p already carries
+    1 / nce_T): b.loss = InfoNCE, and b.g_s / b.g_t = its gradients w.r.t. xs_p / xt_p when allocated.  Only launches on
+    preallocated buffers, so it can be captured."""
+    L, st = _L(), lib.stream_ptr()
+    Sp, Fp = xs_p.shape
+    R = b.Z.shape[0]
+    xt_hi, xt_lo = ops.split_tf32(xt_p, hi=b.xt_split[0], lo=b.xt_split[1])
+    if b.g_s is not None:
+        xtT_hi, xtT_lo = ops.split_tf32(xt_p, transpose=True, hi=b.xtT_split[0], lo=b.xtT_split[1])
+    if b.g_t is not None:
+        b.g_t.zero_()
+    for r0 in range(0, Sp, R):
+        r = min(R, Sp - r0)                                          # multiple of 4
+        Zc = b.Z[:r]
+        ops.gemm_tf32x3(xs_p[r0:r0 + r], xt_hi, xt_lo, out=Zc)
+        if r0 < S:
+            lib.check(L.b200gnn_nce_rows_chunk_f32(_f32(Zc, "Z"), Sp, min(r, S - r0), S, r0, _f32(b.part, "part"), st),
+                      "nce_rows_chunk_f32")
+        if b.g_s is not None:
+            ops.gemm_tf32x3(Zc, xtT_hi, xtT_lo, out=b.g_s[r0:r0 + r])
+        if b.g_t is not None:
+            Ztc = b.Zt[:Sp * r].view(Sp, r)
+            lib.check(L.b200gnn_transpose_f32(_f32(Zc, "Z"), r, Sp, _f32(Ztc, "Zt"), st), "transpose_f32")
+            hi, lo = ops.split_tf32(xs_p[r0:r0 + r], transpose=True, hi=b.xsT_split[0][:Fp * r].view(Fp, r),
+                                    lo=b.xsT_split[1][:Fp * r].view(Fp, r))                  # [Fp, r]
+            ops.gemm_tf32x3(Ztc, hi, lo, out=b.g_t, accumulate=True)
+    lib.check(L.b200gnn_nce_finish_f32(_f32(b.part, "part"), S, _f32(b.loss, "loss"), st), "nce_finish_f32")
+
+
 class _NCE(torch.autograd.Function):
     """InfoNCE between normalised student rows and teacher rows (criterion.py:139-146) WITHOUT the S x S logits tensor
     (1 GiB at the scripts' S = 16384, arxiv_pyg/scripts/run_gcn.sh:144).  The rows are streamed in chunks of R (R*S*4 <=
@@ -409,41 +460,16 @@ class _NCE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fs, ft, nce_T: float):
         fs, ft = fs.contiguous(), ft.contiguous()
-        L, st = _L(), lib.stream_ptr()
         S, F_ = fs.shape
         xs, ns = _normalize(fs, 1.0 / nce_T)          # logits / T folded into the student operand
         xt, nt = _normalize(ft)
         # every matrix is zero-padded to multiples of 4 rows / columns (TMA row pitches): zero feature rows give zero
         # logits, the row pass only visits the S real rows and columns, so the padding never reaches the result
         xs_p, xt_p = _pad_k(_pad_k(xs, 1), 0), _pad_k(_pad_k(xt, 1), 0)
-        Sp, Fp = xs_p.shape
         need_s, need_t = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        R = min(max(128, (NCE_CHUNK_BYTES // (4 * Sp)) // 128 * 128), Sp)
-        xt_hi, xt_lo = ops.split_tf32(xt_p)                              # B of Z_c = xs_c · xt^T         [Sp, Fp]
-        if need_s:
-            xtT_hi, xtT_lo = ops.split_tf32(xt_p, transpose=True)        # B of dZ_c · xt                   [Fp, Sp]
-            g_s = torch.empty(Sp, Fp, device=fs.device)
-        if need_t:
-            g_t = torch.zeros(Sp, Fp, device=fs.device)
-            Zt = _new(Sp * R, like=fs)
-        Z = _new(R, Sp, like=fs)
-        part = _new(S, like=fs)
-        for r0 in range(0, Sp, R):
-            r = min(R, Sp - r0)                                          # multiple of 4
-            Zc = Z[:r]
-            ops.gemm_tf32x3(xs_p[r0:r0 + r], xt_hi, xt_lo, out=Zc)
-            if r0 < S:
-                lib.check(L.b200gnn_nce_rows_chunk_f32(_f32(Zc, "Z"), Sp, min(r, S - r0), S, r0, _f32(part, "part"), st),
-                          "nce_rows_chunk_f32")
-            if need_s:
-                ops.gemm_tf32x3(Zc, xtT_hi, xtT_lo, out=g_s[r0:r0 + r])
-            if need_t:
-                Ztc = Zt[:Sp * r].view(Sp, r)
-                lib.check(L.b200gnn_transpose_f32(_f32(Zc, "Z"), r, Sp, _f32(Ztc, "Zt"), st), "transpose_f32")
-                hi, lo = ops.split_tf32(xs_p[r0:r0 + r], transpose=True)                  # [Fp, r]
-                ops.gemm_tf32x3(Ztc, hi, lo, out=g_t, accumulate=True)
-        loss = _new(1, like=fs)
-        lib.check(L.b200gnn_nce_finish_f32(_f32(part, "part"), S, _f32(loss, "loss"), st), "nce_finish_f32")
+        bufs = NceBuffers(xs_p.shape[0], xs_p.shape[1], fs.device, need_s, need_t)
+        nce_chunks(xs_p, xt_p, S, bufs)
+        loss, g_s, g_t = bufs.loss, bufs.g_s, bufs.g_t
         saved = []
         if need_s:
             saved.append(_normalize_bwd(xs, ns, g_s[:S, :F_], 1.0 / nce_T))

@@ -330,6 +330,28 @@ __global__ void __launch_bounds__(256) affine_relu_bits_kernel(const float* __re
   }
 }
 
+// out[i] = row idx[i] of the hidden activation: X[idx[i]] (pitch ldx), or, with bits, the activation formed from Y, scale,
+// shift and the keep bits exactly as affine_relu_bits_kernel forms it (bit-identical), without the [N, K] matrix.
+__global__ void __launch_bounds__(256) gather_rows_act_kernel(const float* __restrict__ X, int64_t ldx, const int64_t* __restrict__ idx,
+                                                              const uint32_t* __restrict__ bits, const float* __restrict__ scale,
+                                                              const float* __restrict__ shift, float* __restrict__ out,
+                                                              int64_t n_vec, int nvec_row, int words, float p) {
+  const float inv_keep = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / nvec_row;
+    const int cv = (int)(i - r * nvec_row);
+    const int64_t row = __ldg(idx + r);
+    float4 y = ld4(X + row * ldx + 4 * cv);
+    if (bits) {
+      y = affine_relu4(y, scale, shift, cv, 1);
+      const uint32_t b = bits[row * words + (cv >> 3)] >> (4 * (cv & 7));
+      y.x = (b & 1u) ? y.x * inv_keep : 0.f; y.y = (b & 2u) ? y.y * inv_keep : 0.f;
+      y.z = (b & 4u) ? y.z * inv_keep : 0.f; y.w = (b & 8u) ? y.w * inv_keep : 0.f;
+    }
+    st4(out + 4 * i, y);
+  }
+}
+
 // ---------------------------------------------------------------- backward of ReLU+dropout (no BatchNorm)
 // dY = dOut * [Xout > 0] / (1-p)   (the R-GCN's hidden layers: relu -> dropout straight after the conv)
 __global__ void __launch_bounds__(256) relu_dropout_bwd_kernel(const float4* __restrict__ dOut, const float4* __restrict__ Xout,
@@ -645,6 +667,20 @@ extern "C" int b200gnn_affine_relu_bits_f32(const float* Y, const uint32_t* bits
   const int64_t n_vec = n_rows * (K / 4);
   affine_relu_bits_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(Y, bits, scale, shift, out, n_vec,
                                                                                      (int)(K / 4), (int)((K + 31) / 32), p);
+  return check_launch();
+}
+
+extern "C" int b200gnn_gather_rows_act_f32(const float* X, int64_t ldx, const int64_t* idx, int64_t n_idx, int64_t K,
+                                            const uint32_t* bits, const float* scale, const float* shift, float p, float* out,
+                                            void* stream) {
+  if (!rows_ok(n_idx, K) || !X || !idx || !out || ldx < K || ldx % 4 || p < 0.f || p >= 1.f || !aligned_to(X, 16) ||
+      !aligned_to(out, 16))
+    return B200GNN_ERR_BAD_ARG;
+  if (bits && (!scale || !shift || !aligned_to(scale, 16) || !aligned_to(shift, 16))) return B200GNN_ERR_BAD_ARG;
+  if (n_idx == 0) return B200GNN_OK;
+  const int64_t n_vec = n_idx * (K / 4);
+  gather_rows_act_kernel<<<grid_for(n_vec, 256 * 4), 256, 0, (cudaStream_t)stream>>>(X, ldx, idx, bits, scale, shift, out, n_vec,
+                                                                                    (int)(K / 4), (int)((K + 31) / 32), p);
   return check_launch();
 }
 

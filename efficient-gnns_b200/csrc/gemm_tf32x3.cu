@@ -128,6 +128,9 @@ struct Params {
   //                sum (bit ? dA * inv_keep : 0) * z over z <= 0 in fp64 into slope_partial[cta * 8 + warp] (fixed order).
   const float* act_slope;
   double* slope_partial;
+  // ROWIDX: row m of the result is stored to row row_idx[m] of C (the G-CRD head's input gradient, written straight into
+  // the training rows of the [N, H] gradient of the student's last hidden layer).
+  const int64_t* row_idx;
 };
 
 // stat_mode 2: the pieces of Xout / Y one lane needs for a 32-column chunk (4 rows x 4 columns: rows it*4 + lane/8
@@ -170,9 +173,9 @@ __device__ __forceinline__ uint32_t prelu1(uint32_t z, float slope, uint32_t kee
 
 // STAT: 0 plain, 1 / 2 the fused column reductions (Params::stat_mode), 4 the PReLU/dropout backward; PEER: the output goes
 // to peer buffers (Params::Cp); ACT: the hidden activation is recomputed from Y (Params::act_bits); PRELU: the PReLU/dropout
-// prologue.  Compile-time so that each instantiation carries only its own prologue and epilogue (the epilogue is the hot loop
-// of the narrow-K GEMMs).
-template <class C, int STAT, bool PEER, bool ACT = false, bool PRELU = false>
+// prologue; ROWIDX: row-indexed stores (Params::row_idx).  Compile-time so that each instantiation carries only its own
+// prologue and epilogue (the epilogue is the hot loop of the narrow-K GEMMs).
+template <class C, int STAT, bool PEER, bool ACT = false, bool PRELU = false, bool ROWIDX = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                    const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmX,
@@ -412,7 +415,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
               const int r = col0 / p.kc;
               dst = reinterpret_cast<float4*>(p.Cp[r] + (size_t)(p.row_off + grow) * p.kc + (col0 - r * p.kc) + cq);
             } else {
-              dst = reinterpret_cast<float4*>(p.C + (size_t)grow * p.ldc + col0 + cq);
+              const int64_t crow = ROWIDX ? __ldg(p.row_idx + grow) : (int64_t)grow;
+              dst = reinterpret_cast<float4*>(p.C + (size_t)crow * p.ldc + col0 + cq);
             }
             if (!PEER && p.accumulate) { const float4 o = *dst; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
             if (STAT == 1) {
@@ -486,7 +490,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             if (PEER && p.bcast) {
               for (int r = 0; r < p.n_peer; ++r) p.Cp[r][(size_t)(p.row_off + grow) * p.ldc + col] = v;
             } else if (!PEER) {
-              float* dst = p.C + (size_t)grow * p.ldc + col;
+              float* dst = p.C + (size_t)(ROWIDX ? __ldg(p.row_idx + grow) : (int64_t)grow) * p.ldc + col;
               *dst = v + (p.accumulate ? *dst : 0.f);
             }
           }
@@ -544,7 +548,7 @@ static bool make_map(CUtensorMap* m, const float* base, int64_t rows, int64_t co
             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <class C, int STAT = 0, bool PEER = false, bool ACT = false, bool PRELU = false>
+template <class C, int STAT = 0, bool PEER = false, bool ACT = false, bool PRELU = false, bool ROWIDX = false>
 static int launch(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb, const Params& p,
                   cudaStream_t stream) {
   CUtensorMap tA, tBh, tBl, tX, tY;
@@ -559,7 +563,7 @@ static int launch(const float* A, int64_t lda, const float* B_hi, const float* B
   cudaGetDevice(&dev);
   static bool attr_set[64] = {};                    // per device and instantiation; idempotent if two threads race
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU, ROWIDX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          C::SMEM_BYTES);
     if (e != cudaSuccess) { set_cuda_error(e); return B200GNN_ERR_CUDA; }
     attr_set[dev] = true;
@@ -567,7 +571,7 @@ static int launch(const float* A, int64_t lda, const float* B_hi, const float* B
   const int tiles = ((p.M + BM - 1) / BM) * ((p.N + C::BN - 1) / C::BN);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
-  gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
+  gemm_tf32x3_kernel<C, STAT, PEER, ACT, PRELU, ROWIDX><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tA, tBh, tBl, tX, tY, p);
   return check_launch();
 }
 
@@ -763,6 +767,23 @@ extern "C" int b200gnn_gemm_tf32x3_f32(const float* A, int64_t lda, const float*
 extern "C" int b200gnn_gemm_tf32x3_acc_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
                                            float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, void* stream) {
   return gemm_dispatch(A, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, nullptr, 1, stream);
+}
+
+// C[row_idx[m]] = (A · B^T)[m]: the result's rows stored to the C rows row_idx names (int64, distinct, each < the rows of
+// C; rows not named are left as they are).  The G-CRD step's student-head input gradient: dP_s · W_s for the n_train
+// rows lands in the training rows of the [N, H] gradient of out_feat (arxiv_pyg/gnn.py:296 student_proj(out_feat[train_idx])).
+extern "C" int b200gnn_gemm_tf32x3_rowidx_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                              float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const int64_t* row_idx,
+                                              void* stream) {
+  if (!A || !B_hi || !B_lo || !C || !row_idx || M <= 0 || N <= 0 || K <= 0 || lda < K || ldb < K || ldc < N ||
+      M >= INT32_MAX || N >= INT32_MAX || K >= INT32_MAX)
+    return B200GNN_ERR_BAD_ARG;
+  if (lda % 4 || ldb % 4 || !aligned_to(A, 16) || !aligned_to(B_hi, 16) || !aligned_to(B_lo, 16)) return B200GNN_ERR_UNSUPPORTED;
+  gemm::Params p{};
+  p.C = C; p.bias = nullptr; p.ldc = ldc; p.M = (int32_t)M; p.N = (int32_t)N; p.K = (int32_t)K; p.accumulate = 0;
+  p.row_idx = row_idx;
+  if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>, 0, false, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+  return gemm::launch<gemm::Cfg<128, 4>, 0, false, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
 }
 
 // C = A · B^T (+bias) with the output SCATTERED BY COLUMN BLOCK to `world` destination buffers: columns [q*kc, (q+1)*kc)

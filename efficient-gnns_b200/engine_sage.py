@@ -31,7 +31,8 @@ from .sparse import CsrGraph, SparseTensor
 class SAGEStudentTrainer:
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
-                 fuse_row_passes: bool = True):
+                 fuse_row_passes: bool = True, gcrd=None):
+        """gcrd: a gcrd.GCRD run inside the step as engine.GCNStudentTrainer runs it; None leaves the step as it is."""
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         for d in dims:
             assert d % 4 == 0 and d <= 1024, "layer widths must be multiples of 4 (128-bit rows)"
@@ -95,6 +96,9 @@ class SAGEStudentTrainer:
         self.loss_aux = None
         self._graph = None
         self.reset_parameters(seed)
+        self.gcrd = gcrd
+        if gcrd is not None:
+            gcrd.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def reset_parameters(self, seed: int = 0):
@@ -237,17 +241,28 @@ class SAGEStudentTrainer:
         ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],
                             loss_out=self.loss_out, partial=self.kd_part)
 
-    def _step_impl(self, x, y, train_idx, teacher_logits):
+    def _step_impl(self, x, y, train_idx, teacher_logits, sample=None):
         self._loss(x, y, train_idx, teacher_logits)
-        self.backward(x)
+        if self.gcrd is None:
+            self.backward(x)
+            ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
+            return
+        self.backward(x, d_out_feat=self.gcrd.forward_backward(self, sample))
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
+        self.gcrd.optimizer_step(self.lr)
 
-    def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0) -> torch.Tensor:
+    def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
+                   sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One reference ``train()`` call for ``--gnn sage``: supervised / kd, or kd + beta*aux with ``aux(out_feat)`` as in
-        engine.GCNStudentTrainer.train_step.  Returns the device tensor [loss, loss_cls, loss_kd]."""
+        engine.GCNStudentTrainer.train_step, or with the G-CRD object of the constructor (``sample`` as there).  Returns the
+        device tensor [loss, loss_cls, loss_kd]."""
+        if sample is not None and self.gcrd is None:
+            raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
         if aux is None:
-            self._step_impl(x, y, train_idx, teacher_logits)
+            self._step_impl(x, y, train_idx, teacher_logits, *(() if sample is None else (sample,)))
             return self.loss_out
+        if self.gcrd is not None:
+            raise ValueError("aux= and a G-CRD head are two auxiliary losses; pass one")
         self._loss(x, y, train_idx, teacher_logits)
         feat = self.out_feat().detach().requires_grad_(True)
         with torch.enable_grad():

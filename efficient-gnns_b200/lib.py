@@ -60,6 +60,7 @@ SIGNATURES = {
     "b200gnn_dropout_mask_step_u8": (_int, [_ptr, _i64, _i64, _f32, _u64, _u64, _i32p, _u64, _ptr]),
     "b200gnn_dropout_bits_u32": (_int, [_ptr, _i64, _i64, _i64, _f32, _u64, _u64, _i32p, _u64, _ptr]),
     "b200gnn_affine_relu_bits_f32": (_int, [_f32p, _ptr, _f32p, _f32p, _f32, _f32p, _i64, _i64, _ptr]),
+    "b200gnn_gather_rows_act_f32": (_int, [_f32p, _i64, _ptr, _i64, _i64, _ptr, _f32p, _f32p, _f32, _f32p, _ptr]),
     "b200gnn_relu_dropout_bwd_f32": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _f32, _ptr]),
     "b200gnn_bn_act_bwd_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32, _f32p, _f32p,
                                       _f32p, _f32p, _f32p, _i64, _f32p, _ptr]),
@@ -96,6 +97,7 @@ SIGNATURES = {
     "b200gnn_gemm_tf32x3_act_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p,
                                            _f32p, _f32p, _ptr, _f32, _ptr]),
     "b200gnn_gemm_tf32x3_acc_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _ptr]),
+    "b200gnn_gemm_tf32x3_rowidx_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _ptr, _ptr]),
     "b200gnn_gemm_tf32x3_scatter_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gemm_tf32x3_bcast_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _ptr, _i32, _i64, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_wgrad_workspace_floats": (_i64, [_i64, _i64]),
@@ -123,6 +125,13 @@ SIGNATURES = {
     "b200gnn_nce_rows_f32": (_int, [_f32p, _i64, _f32p, _f32p, _ptr]),
     "b200gnn_nce_rows_chunk_f32": (_int, [_f32p, _i64, _i64, _i64, _i64, _f32p, _ptr]),
     "b200gnn_nce_finish_f32": (_int, [_f32p, _i64, _f32p, _ptr]),
+    "b200gnn_gcrd_sample_workspace_bytes": (_i64, [_i64]),
+    "b200gnn_gcrd_sample_i32": (_int, [_i64, _u64, _u64, _i32p, _i32p, _ptr, _ptr]),
+    "b200gnn_gcrd_operands_f32": (_int, [_i32p, _i64, _i64, _f32p, _f32p, _f32p, _f32p, _f32, _f32, _f32p, _f32p, _f32p, _f32p,
+                                         _ptr]),
+    "b200gnn_gcrd_bwd_slots": (_i64, []),
+    "b200gnn_gcrd_backward_f32": (_int, [_i32p, _i64, _i64, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32, _f32, _f32p, _f32p,
+                                         _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_transpose_f32": (_int, [_f32p, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gsp_pair_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _int, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_row_axpy_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32, _f32p, _ptr]),

@@ -239,6 +239,19 @@ def affine_relu_bits(y: torch.Tensor, bits: torch.Tensor, scale: torch.Tensor, s
     return out
 
 
+def gather_rows_act(x: torch.Tensor, idx: torch.Tensor, out: torch.Tensor, bits: Optional[torch.Tensor] = None,
+                    scale: Optional[torch.Tensor] = None, shift: Optional[torch.Tensor] = None, p: float = 0.0) -> torch.Tensor:
+    """out[i] = x[idx[i]] (idx int64), or with ``bits`` the activation dropout(relu(x[idx[i]]*scale + shift)) of
+    ``affine_relu_bits`` (bit-identical) without materialising it for every row."""
+    n, K = out.shape
+    assert x.shape[1] == K and idx.numel() == n
+    lib.check(lib.load().b200gnn_gather_rows_act_f32(
+        _f32(x, "x"), x.stride(0), lib.dptr(idx, torch.int64, "idx"),
+        n, K, None if bits is None else _bits(bits, x.shape[0], K), _f32(scale, "scale"), _f32(shift, "shift"), float(p),
+        _f32(out, "out"), lib.stream_ptr()), "gather_rows_act_f32")
+    return out
+
+
 def bn_act_bwd(d_out, x_out, y, mean, invstd, gamma, p: float, d_y=None, d_gamma=None, d_beta=None, d_bias=None,
                partial=None, coef=None, want_dbias: bool = True):
     """Backward of x_out = dropout_p(relu(BN_train(y))). Returns (d_y, d_gamma, d_beta, d_bias)."""
@@ -390,6 +403,19 @@ def gemm_tf32x3_act(y: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, b
                                                      b_hi.stride(0), _f32(out, "out"), out.stride(0), M, N, K, _f32(bias, "bias"),
                                                      _f32(scale, "scale"), _f32(shift, "shift"), _bits(bits, M, K), float(p),
                                                      lib.stream_ptr()), "gemm_tf32x3_act_f32")
+    return out
+
+
+def gemm_tf32x3_rowidx(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, out: torch.Tensor,
+                       row_idx: torch.Tensor) -> torch.Tensor:
+    """out[row_idx[m]] = (a @ b^T)[m] (row_idx int64, distinct); rows of out that row_idx does not name are left as they are."""
+    M, K = a.shape
+    N = b_hi.shape[0]
+    assert b_hi.shape == b_lo.shape and b_hi.shape[1] == K and row_idx.numel() == M and out.shape[1] == N
+    lib.check(lib.load().b200gnn_gemm_tf32x3_rowidx_f32(_f32(a, "a"), a.stride(0), _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"),
+                                                        b_hi.stride(0), _f32(out, "out"), out.stride(0), M, N, K,
+                                                        lib.dptr(row_idx, torch.int64, "row_idx"), lib.stream_ptr()),
+              "gemm_tf32x3_rowidx_f32")
     return out
 
 

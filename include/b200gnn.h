@@ -201,6 +201,13 @@ int b200gnn_dropout_bits_u32(uint32_t* bits, int64_t n_layers, int64_t n_rows, i
                              uint64_t offset, const int32_t* step_dev, uint64_t step_mul, void* stream);
 int b200gnn_affine_relu_bits_f32(const float* Y, const uint32_t* bits, const float* scale, const float* shift,
                                  float p, float* out, int64_t n_rows, int64_t K, void* stream);
+/* out[i] = row idx[i] (int64) of a hidden activation, [n_idx, K] contiguous: X[idx[i]] (row pitch ldx), or, with bits
+ * (uint32 [rows][ceil(K/32)] of b200gnn_dropout_bits_u32), dropout(relu(X[idx[i]] * scale + shift)) formed exactly as
+ * b200gnn_affine_relu_bits_f32 forms it (bit-identical).  The G-CRD step's model.out_feat[train_idx]
+ * (arxiv_pyg/gnn.py:296) without the [N, K] activation. */
+int b200gnn_gather_rows_act_f32(const float* X, int64_t ldx, const int64_t* idx, int64_t n_idx, int64_t K,
+                                const uint32_t* bits, const float* scale, const float* shift, float p, float* out,
+                                void* stream);
 /* Backward of out = dropout_p(relu(Y)) (no BatchNorm): dY = dOut * [Xout > 0] / (1-p), contiguous [n_rows, K]
  * rows, K a multiple of 4; dY may alias dOut. */
 int b200gnn_relu_dropout_bwd_f32(const float* dOut, const float* Xout, float* dY,
@@ -332,6 +339,11 @@ int b200gnn_gemm_tf32x3_f32(const float* A, int64_t lda, const float* B_hi,
 int b200gnn_gemm_tf32x3_acc_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo,
                                 int64_t ldb, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
                                 void* stream);
+/* C[row_idx[m]] = (A · B^T)[m]: row-indexed stores (row_idx int64, distinct); C rows not named are untouched.  The G-CRD
+ * student head's input gradient stored into the training rows of d out_feat (arxiv_pyg/gnn.py:296). */
+int b200gnn_gemm_tf32x3_rowidx_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo,
+                                   int64_t ldb, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                                   const int64_t* row_idx, void* stream);
 /* Row passes fused into the GEMM epilogue (SURVEY §8 f1; the reference runs conv -> BatchNorm1d -> ReLU -> dropout as
  * separate full-matrix ops, arxiv_pyg/gnn.py:47-50, and autograd walks them again backwards).  Each consumer warp keeps
  * running column sums over the tiles of its CTA and stores them once: partial[slots][2][N], slots >=
@@ -478,6 +490,29 @@ int b200gnn_nce_rows_f32(float* Z, int64_t S, float* loss_out, float* partial, v
 int b200gnn_nce_rows_chunk_f32(float* Z, int64_t ldz, int64_t n_rows, int64_t S, int64_t row_offset,
                                float* partial, void* stream);
 int b200gnn_nce_finish_f32(const float* partial, int64_t S, float* loss_out, void* stream);
+/* The captured G-CRD step (csrc/gcrd.cu; nce_criterion :129-149 on the projection heads of arxiv_pyg/gnn.py:296-306).
+ *   gcrd_sample: perm_out[n] = the n training-row positions ordered by (Philox key, position), keys drawn at
+ *     (seed, offset + *step_dev); its first S entries are the step's sample of S distinct rows (np.random.choice(n, S,
+ *     replace=False) at criterion.py:135, drawn on the device).  workspace: b200gnn_gcrd_sample_workspace_bytes(n).
+ *   gcrd_operands: x_s[j] = relu(bn_s(pre_s[inds[j]])) normalised and scaled by inv_T, x_t[j] the same for the teacher
+ *     head unscaled (F.normalize, eps), norms to norm_s / norm_t; pre_* [n_train, P], bn_* [4][P] (mean, invstd, scale,
+ *     shift), x_* [S, P]; P a multiple of 4, at most 256.
+ *   gcrd_backward: from g_* = d loss / d x_* ([S, P]) to dz_* = beta * d loss / d (bn output) at rows inds[j] of the
+ *     zero-filled [n_train, P] dz_* (normalise backward, ReLU mask), and pass 1 of the BatchNorm backward: part_*[slots][2][P]
+ *     (slots = b200gnn_gcrd_bwd_slots()) = per-warp (sum dz, sum dz * xhat) for b200gnn_bn_act_bwd_apply_f32 with Xout = NULL.
+ *     loss_total[0] += beta * loss_aux[0] when loss_total is given. */
+int64_t b200gnn_gcrd_sample_workspace_bytes(int64_t n);
+int b200gnn_gcrd_sample_i32(int64_t n, uint64_t seed, uint64_t offset, const int32_t* step_dev, int32_t* perm_out,
+                            void* workspace, void* stream);
+int b200gnn_gcrd_operands_f32(const int32_t* inds, int64_t S, int64_t P, const float* pre_s, const float* bn_s,
+                              const float* pre_t, const float* bn_t, float inv_T, float eps, float* x_s, float* x_t,
+                              float* norm_s, float* norm_t, void* stream);
+int64_t b200gnn_gcrd_bwd_slots(void);
+int b200gnn_gcrd_backward_f32(const int32_t* inds, int64_t S, int64_t P, const float* g_s, const float* g_t,
+                              const float* x_s, const float* x_t, const float* norm_s, const float* norm_t, float inv_T,
+                              float eps, const float* pre_s, const float* bn_s, const float* pre_t, const float* bn_t,
+                              float beta, float* dz_s, float* dz_t, float* part_s, float* part_t, const float* loss_aux,
+                              float* loss_total, void* stream);
 int b200gnn_transpose_f32(const float* in, int64_t rows, int64_t cols, float* out, void* stream);
 /* GSP (gpw_criterion :66-86): Gs/Gt = Gram matrices of the sampled student/teacher rows; kernel 0 cosine,
  * 1 poly, 2 l2, 3 rbf (ns/nt = row squared norms for 2,3).  loss_out[0] = mse(sim_s, sim_t); Gs is overwritten by
