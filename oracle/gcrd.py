@@ -5,9 +5,21 @@ from __future__ import annotations
 
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import criterion as oc, nn as onn
+from .sampling import philox4x32
+
+
+def sample_perm(n: int, seed: int, offset: int, tie_to_higher: bool = False) -> np.ndarray:
+    """The on-device row sample (b200gnn_gcrd_sample_i32) restated: row i gets key word i % 4 of
+    philox4x32(seed, offset, i >> 2), and the rows are ordered by (key, row), so equal keys go to the lower row.  The first
+    S entries are a step's sample.  tie_to_higher orders equal keys the other way (a control for tests only).  -> int64 [n]."""
+    words = philox4x32(seed, offset % (1 << 64), np.arange((n + 3) // 4, dtype=np.uint64))
+    key = words.reshape(-1)[:n].astype(np.int64)
+    row = np.arange(n, dtype=np.int64)
+    return np.lexsort((n - 1 - row if tie_to_higher else row, key)).astype(np.int64)
 
 
 def _head(f, sd, eps):

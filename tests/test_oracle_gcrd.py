@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from oracle import gcrd as og_gcrd, graph as og
+from oracle.sampling import philox4x32
 
 GOLD = Path(__file__).resolve().parent / "golden" / "gcrd_arxiv.pt"
 CASES = ["gnn_gcn", "gnn_sage", "kd_and_aux_gcn", "kd_and_aux_sage"]
@@ -68,3 +69,32 @@ def test_oracle_reproduces_the_reference_train_step(gold, name):
             if "num_batches" in k or pre_bn_bias(group, k) or (group == "model" and "running" in k):
                 continue
             assert rel(ref["after"][group][k], v) < 1e-5, (name, group, k)
+
+
+def _seed_with_tie(n, offset):
+    """The first seed whose n keys at this offset contain an equal pair (about 60 % of seeds at n = 90,941)."""
+    for seed in range(64):
+        key = philox4x32(seed, offset, np.arange((n + 3) // 4, dtype=np.uint64)).reshape(-1)[:n]
+        if np.unique(key).size < n:
+            return seed, key.astype(np.int64)
+    raise AssertionError("no tied keys in 64 seeds")
+
+
+def test_sample_perm_is_a_permutation_ordered_by_key_then_row():
+    """oracle/gcrd.sample_perm: a permutation of [0, n), keys nondecreasing along it, and equal keys in ascending row order;
+    the tie_to_higher control orders the same tie the other way, so it differs exactly where a tie is."""
+    n, offset = 90_941, 1 << 62
+    seed, key = _seed_with_tie(n, offset)
+    perm = og_gcrd.sample_perm(n, seed, offset)
+    assert perm.dtype == np.int64 and np.array_equal(np.sort(perm), np.arange(n))
+    k = key[perm]
+    assert (np.diff(k) >= 0).all()
+    tied = np.flatnonzero(np.diff(k) == 0)
+    assert tied.size > 0 and (perm[tied] < perm[tied + 1]).all()
+    ctrl = og_gcrd.sample_perm(n, seed, offset, tie_to_higher=True)
+    assert np.array_equal(key[ctrl], k) and (ctrl[tied] > ctrl[tied + 1]).all()
+    assert not np.array_equal(ctrl, perm)
+    # small n, and word i % 4 of block i >> 2: n = 5 uses block 1's first word for row 4
+    w = philox4x32(3, 7, np.arange(2, dtype=np.uint64)).reshape(-1)
+    assert np.array_equal(og_gcrd.sample_perm(5, 3, 7), np.argsort(w[:5], kind="stable"))
+    assert np.array_equal(og_gcrd.sample_perm(1, 3, 7), [0])
