@@ -198,6 +198,136 @@ __global__ void __launch_bounds__(256) lsp_diag_kernel(const int32_t* __restrict
   }
 }
 
+// The student side of the captured LSP step (criterion kld): edge_sim(student) -> lsp_segment -> lsp_edge_coef in one
+// kernel, one warp per destination segment with lsp_segment_kernel's grid and warp-to-segment mapping, so every float it
+// produces is the one the three kernels produce (same per-lane fmaf chains, same butterflies, same per-lane edge order).
+//   pass 1: per edge, the whole warp forms k(f[src], f[dst]) as edge_sim_kernel does; the destination row (the same for the
+//           whole segment) sits in registers, NC floats per lane (F <= 32 NC), and its squared norm is reduced once.
+//           sim_s[e] and, for cosine / poly, c[e] and the unclamped source norm ra[e] go to memory.
+//   pass 2 + 3: lane-per-edge, lsp_segment_kernel's statistics and KL terms, then g_e and lsp_edge_coef_kernel's w / sa / sb
+//           from the pass-1 terms, without reading the features again.
+template <int NC>
+__global__ void __launch_bounds__(256, 4) lsp_student_kernel(const float* __restrict__ feat, int F, const int32_t* __restrict__ src,
+                                                          const int32_t* __restrict__ dst, const int32_t* __restrict__ rowptr,
+                                                          int64_t n_seg, const float* __restrict__ sim_t, int kernel,
+                                                          float inv_E, const int32_t* __restrict__ pos_dst,
+                                                          const int32_t* __restrict__ pos_src, float* sim_s, float* c_e,
+                                                          float* ra_e, float* __restrict__ val, float* __restrict__ selfc,
+                                                          float* __restrict__ partial) {
+  __shared__ float s_acc[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float acc = 0.f;
+  for (int64_t i = (int64_t)blockIdx.x * 8 + warp; i < n_seg; i += (int64_t)gridDim.x * 8) {
+    const int b = rowptr[i], e = rowptr[i + 1];
+    if (b == e) continue;
+    // ---- pass 1
+    const float* brow = feat + (size_t)dst[b] * F;
+    float yr[NC];
+#pragma unroll
+    for (int j = 0; j < NC; ++j) yr[j] = lane + 32 * j < F ? __ldg(brow + lane + 32 * j) : 0.f;
+    float rb = 0.f, nb = 0.f;
+    if (kernel <= 1) {
+      float nb2 = 0.f;
+#pragma unroll
+      for (int j = 0; j < NC; ++j)
+        if (lane + 32 * j < F) nb2 = fmaf(yr[j], yr[j], nb2);
+      rb = sqrtf(wsum(nb2));
+      nb = fmaxf(rb, COS_EPS);
+    }
+    for (int k = b; k < e; ++k) {
+      const float* a = feat + (size_t)src[k] * F;
+      float s;
+      if (kernel <= 1) {
+        float dot = 0.f, na2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < NC; ++j)
+          if (lane + 32 * j < F) { const float x = __ldg(a + lane + 32 * j); dot = fmaf(x, yr[j], dot); na2 = fmaf(x, x, na2); }
+        dot = wsum(dot); na2 = wsum(na2);
+        const float ra = sqrtf(na2);
+        const float c = dot / (fmaxf(ra, COS_EPS) * nb);
+        s = kernel == 0 ? c : c * c;
+        if (lane == 0) { c_e[k] = c; ra_e[k] = ra; }
+      } else {
+        float d2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < NC; ++j)
+          if (lane + 32 * j < F) { const float d = __ldg(a + lane + 32 * j) - yr[j]; d2 = fmaf(d, d, d2); }
+        d2 = wsum(d2);
+        s = kernel == 2 ? sqrtf(d2) : expf(-0.5f * d2);
+      }
+      if (lane == 0) sim_s[k] = s;
+    }
+    __syncwarp();                                   // lane 0's stores above are read by every lane below
+    // ---- pass 2: lsp_segment_kernel, criterion 0
+    float ms = -INFINITY, mt = -INFINITY;
+    for (int k = b + lane; k < e; k += 32) { ms = fmaxf(ms, sim_s[k]); mt = fmaxf(mt, sim_t[k]); }
+    ms = wmax(ms); mt = wmax(mt);
+    float zs = 0.f, zt = 0.f;
+    for (int k = b + lane; k < e; k += 32) { zs += expf(sim_s[k] - ms); zt += expf(sim_t[k] - mt); }
+    zs = wsum(zs) + 1e-16f; zt = wsum(zt) + 1e-16f;
+    const float lzs = logf(zs), lzt = logf(zt);
+    const float T = (zt - 1e-16f) / zt;
+    for (int k = b + lane; k < e; k += 32) {
+      const float sk = sim_s[k];
+      const float lps = (sk - ms) - lzs, lpt = (sim_t[k] - mt) - lzt;
+      const float ps = expf(lps), pt = expf(lpt);
+      acc += pt > 0.f ? pt * (lpt - lps) : 0.f;
+      float ge = (ps * T - pt) * inv_E;
+      // ---- pass 3: lsp_edge_coef_kernel from the pass-1 terms
+      float w, sa, sb;
+      if (kernel <= 1) {
+        const float c = c_e[k], ra = ra_e[k];
+        const float na = fmaxf(ra, COS_EPS);
+        if (kernel == 1) ge *= 2.f * c;
+        w = ge / (na * nb);
+        sa = ra > COS_EPS ? ge * c / (na * na) : 0.f;   // clamped norm carries no gradient
+        sb = rb > COS_EPS ? ge * c / (nb * nb) : 0.f;
+      } else {
+        float coef;
+        if (kernel == 2) coef = sk > 0.f ? ge / sk : 0.f;
+        else coef = -ge * sk;
+        w = -coef; sa = -coef; sb = -coef;
+      }
+      const int pd = pos_dst[k], pq = pos_src[k];
+      val[pd] = w; selfc[pd] = sb;
+      val[pq] = w; selfc[pq] = sa;
+    }
+  }
+  acc = wsum(acc);
+  if (lane == 0) s_acc[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += s_acc[w];
+    partial[blockIdx.x] = t;
+  }
+}
+
+// dst[idx[i]] = src[i] * scale (a plain fp32 product), one warp per row; thread 0 of block 0 also forms
+// loss_total[0] += loss_aux[0] * scale (fp32 product, then fp32 add) when loss_total is given.
+template <bool VEC>
+__global__ void __launch_bounds__(256) scatter_rows_scaled_kernel(const float* __restrict__ src, const int64_t* __restrict__ idx,
+                                                                  int64_t n, int K, float scale, float* __restrict__ dst,
+                                                                  int64_t ldd, const float* __restrict__ loss_aux,
+                                                                  float* __restrict__ loss_total) {
+  if (loss_total && blockIdx.x == 0 && threadIdx.x == 0) loss_total[0] = __fadd_rn(loss_total[0], __fmul_rn(loss_aux[0], scale));
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5), nwarps = (int64_t)gridDim.x * 8;
+  for (int64_t i = warp; i < n; i += nwarps) {
+    const float* s = src + (size_t)i * K;
+    float* d = dst + (size_t)idx[i] * ldd;
+    if (VEC) {
+      for (int k = lane; k < K / 4; k += 32) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(s) + k);
+        reinterpret_cast<float4*>(d)[k] = make_float4(__fmul_rn(v.x, scale), __fmul_rn(v.y, scale), __fmul_rn(v.z, scale),
+                                                      __fmul_rn(v.w, scale));
+      }
+    } else {
+      for (int k = lane; k < K; k += 32) d[k] = __fmul_rn(__ldg(s + k), scale);
+    }
+  }
+}
+
 static inline int edge_grid(int64_t items) {
   int64_t g = (items + 7) / 8;
   if (g > 132 * 16) g = 132 * 16;
@@ -258,5 +388,52 @@ extern "C" int b200gnn_lsp_bwd_values_f32(const float* feat, int64_t F, const in
     if ((rc = check_launch())) return rc;
   }
   lsp_diag_kernel<<<edge_grid(n_nodes), 256, 0, st>>>(comb_rowptr, diag_pos, n_nodes, selfc, val);
+  return check_launch();
+}
+
+// The captured LSP step's student side (kld): lsp_student_kernel, then lsp_diag_kernel and sum_partials_kernel, with the
+// launches and grids of edge_sim -> lsp_segment -> lsp_bwd_values.  scratch: 2E floats (c and ra per edge).
+extern "C" int b200gnn_lsp_student_f32(const float* feat, int64_t F, const int32_t* src, const int32_t* dst,
+                                       const int32_t* rowptr, int64_t n_seg, int64_t E, const float* sim_t, int kernel,
+                                       const int32_t* pos_dst, const int32_t* pos_src, const int32_t* comb_rowptr,
+                                       const int32_t* diag_pos, int64_t n_nodes, float* sim_s, float* scratch, float* val,
+                                       float* selfc, float* loss_out, float* partial, void* stream) {
+  if (!feat || !src || !dst || !rowptr || !sim_t || !pos_dst || !pos_src || !comb_rowptr || !diag_pos || !sim_s || !scratch ||
+      !val || !selfc || !loss_out || !partial || F <= 0 || F > B200GNN_LSP_MAX_F || E <= 0 || n_seg <= 0 || n_nodes <= 0 ||
+      kernel < 0 || kernel > 3)
+    return B200GNN_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = edge_grid(n_seg);
+  const float inv_E = 1.f / (float)E;
+  float *c_e = scratch, *ra_e = scratch + E;
+#define LSP_STUDENT(NC) \
+  lsp_student_kernel<NC><<<grid, 256, 0, st>>>(feat, (int)F, src, dst, rowptr, n_seg, sim_t, kernel, inv_E, pos_dst, pos_src, \
+                                               sim_s, c_e, ra_e, val, selfc, partial)
+  if (F <= 32) LSP_STUDENT(1);
+  else if (F <= 64) LSP_STUDENT(2);
+  else if (F <= 128) LSP_STUDENT(4);
+  else if (F <= 256) LSP_STUDENT(8);
+  else LSP_STUDENT(16);
+#undef LSP_STUDENT
+  int rc;
+  if ((rc = check_launch())) return rc;
+  lsp_diag_kernel<<<edge_grid(n_nodes), 256, 0, st>>>(comb_rowptr, diag_pos, n_nodes, selfc, val);
+  if ((rc = check_launch())) return rc;
+  sum_partials_kernel<<<1, 256, 0, st>>>(partial, grid, 1.0 / (double)E, loss_out);
+  return check_launch();
+}
+
+extern "C" int b200gnn_scatter_rows_scaled_f32(const float* src, const int64_t* idx, int64_t n, int64_t K, float scale,
+                                               float* dst, int64_t ldd, const float* loss_aux, float* loss_total,
+                                               void* stream) {
+  if (!src || !idx || !dst || n < 0 || K <= 0 || K > INT32_MAX || ldd < K || (loss_total && !loss_aux))
+    return B200GNN_ERR_BAD_ARG;
+  if (n == 0 && !loss_total) return B200GNN_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = edge_grid(n);
+  if (K % 4 == 0 && ldd % 4 == 0 && aligned_to(src, 16) && aligned_to(dst, 16))
+    scatter_rows_scaled_kernel<true><<<grid, 256, 0, st>>>(src, idx, n, (int)K, scale, dst, ldd, loss_aux, loss_total);
+  else
+    scatter_rows_scaled_kernel<false><<<grid, 256, 0, st>>>(src, idx, n, (int)K, scale, dst, ldd, loss_aux, loss_total);
   return check_launch();
 }

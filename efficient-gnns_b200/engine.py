@@ -54,9 +54,12 @@ class GCNStudentTrainer:
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
                  aggregate_first: Optional[bool] = None, tensor_core_gemm: bool = True, overlap_wgrad: bool = True,
                  fuse_row_passes: bool = True, fuse_activations: bool = True, _prebuilt_graph: Optional[CsrGraph] = None, _rows_alloc: Optional[int] = None,
-                 gcrd=None):
+                 gcrd=None, lsp=None):
         """gcrd: a gcrd.GCRD whose projection heads and InfoNCE loss run inside this trainer's step (kd or supervised + beta *
-        G-CRD, one CUDA graph); None leaves the step as it is."""
+        G-CRD, one CUDA graph); lsp: an lsp.LSP run the same way (kd or supervised + beta * LSP); None for both leaves the step
+        as it is."""
+        if gcrd is not None and lsp is not None:
+            raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         self.device = adj.device
         self.dims, self.L = list(dims), len(dims) - 1
@@ -181,9 +184,9 @@ class GCNStudentTrainer:
         self._static: Dict[str, torch.Tensor] = {}
         for k in set(dims[1:]):
             self._part(k); self._coef(k)
-        self.gcrd = gcrd
-        if gcrd is not None:
-            gcrd.bind(self)
+        self.objective = gcrd if gcrd is not None else lsp      # the auxiliary loss run inside the step, if any
+        if self.objective is not None:
+            self.objective.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def reset_parameters(self, seed: int = 0):
@@ -421,13 +424,13 @@ class GCNStudentTrainer:
         self.dY[-1].zero_()
         ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],
                             loss_out=self.loss_out, partial=self.kd_part)
-        if self.gcrd is None:
+        if self.objective is None:
             self.backward(x)
             ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
             return
-        self.backward(x, d_out_feat=self.gcrd.forward_backward(self, sample))
+        self.backward(x, d_out_feat=self.objective.forward_backward(self, sample))
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.gcrd.optimizer_step(self.lr)
+        self.objective.optimizer_step(self.lr)
 
     def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
                    sample: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -437,15 +440,15 @@ class GCNStudentTrainer:
         ``lambda f: criterion.lpw_criterion(z, y, f[idx], t_feat[idx], edge_index, "cosine", 1)[2]`` or a projection head +
         ``nce_criterion``; parameters of such heads get their gradients through torch autograd and stay with the caller's
         optimizer.  Returns the device tensor [loss, loss_cls, loss_kd] (+ beta*aux folded into loss); no host sync.
-        With a G-CRD object (constructor) the step includes it (loss[0] += beta * G-CRD, value in gcrd.loss_aux);
-        ``sample`` (positions into train_idx, [S]) then replaces the step's on-device row draw."""
-        if sample is not None and self.gcrd is None:
+        With a G-CRD or LSP object (constructor) the step includes it (loss[0] += beta * loss_aux, value in its loss_aux);
+        ``sample`` (positions into train_idx, [S]) then replaces G-CRD's on-device row draw."""
+        if sample is not None and self.objective is None:
             raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
         if aux is None:
             self._step_impl(x, y, train_idx, teacher_logits, *(() if sample is None else (sample,)))
             return self.loss_out
-        if self.gcrd is not None:
-            raise ValueError("aux= and a G-CRD head are two auxiliary losses; pass one")
+        if self.objective is not None:
+            raise ValueError("aux= and the trainer's G-CRD / LSP objective are two auxiliary losses; pass one")
         logits = self.forward(x, training=True)
         self.dY[-1].zero_()
         ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],

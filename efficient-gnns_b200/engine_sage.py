@@ -31,8 +31,11 @@ from .sparse import CsrGraph, SparseTensor
 class SAGEStudentTrainer:
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
-                 fuse_row_passes: bool = True, gcrd=None):
-        """gcrd: a gcrd.GCRD run inside the step as engine.GCNStudentTrainer runs it; None leaves the step as it is."""
+                 fuse_row_passes: bool = True, gcrd=None, lsp=None):
+        """gcrd / lsp: a gcrd.GCRD or an lsp.LSP run inside the step as engine.GCNStudentTrainer runs it; None for both
+        leaves the step as it is."""
+        if gcrd is not None and lsp is not None:
+            raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         for d in dims:
             assert d % 4 == 0 and d <= 1024, "layer widths must be multiples of 4 (128-bit rows)"
@@ -96,9 +99,9 @@ class SAGEStudentTrainer:
         self.loss_aux = None
         self._graph = None
         self.reset_parameters(seed)
-        self.gcrd = gcrd
-        if gcrd is not None:
-            gcrd.bind(self)
+        self.objective = gcrd if gcrd is not None else lsp      # the auxiliary loss run inside the step, if any
+        if self.objective is not None:
+            self.objective.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def reset_parameters(self, seed: int = 0):
@@ -243,26 +246,26 @@ class SAGEStudentTrainer:
 
     def _step_impl(self, x, y, train_idx, teacher_logits, sample=None):
         self._loss(x, y, train_idx, teacher_logits)
-        if self.gcrd is None:
+        if self.objective is None:
             self.backward(x)
             ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
             return
-        self.backward(x, d_out_feat=self.gcrd.forward_backward(self, sample))
+        self.backward(x, d_out_feat=self.objective.forward_backward(self, sample))
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.gcrd.optimizer_step(self.lr)
+        self.objective.optimizer_step(self.lr)
 
     def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
                    sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One reference ``train()`` call for ``--gnn sage``: supervised / kd, or kd + beta*aux with ``aux(out_feat)`` as in
-        engine.GCNStudentTrainer.train_step, or with the G-CRD object of the constructor (``sample`` as there).  Returns the
-        device tensor [loss, loss_cls, loss_kd]."""
-        if sample is not None and self.gcrd is None:
+        engine.GCNStudentTrainer.train_step, or with the G-CRD or LSP object of the constructor (``sample`` as there).  Returns
+        the device tensor [loss, loss_cls, loss_kd]."""
+        if sample is not None and self.objective is None:
             raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
         if aux is None:
             self._step_impl(x, y, train_idx, teacher_logits, *(() if sample is None else (sample,)))
             return self.loss_out
-        if self.gcrd is not None:
-            raise ValueError("aux= and a G-CRD head are two auxiliary losses; pass one")
+        if self.objective is not None:
+            raise ValueError("aux= and the trainer's G-CRD / LSP objective are two auxiliary losses; pass one")
         self._loss(x, y, train_idx, teacher_logits)
         feat = self.out_feat().detach().requires_grad_(True)
         with torch.enable_grad():

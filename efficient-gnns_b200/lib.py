@@ -17,6 +17,7 @@ LIB_PATH = PKG_DIR / "libb200gnn.so"
 OK = 0
 REDUCE_SUM = 0
 REDUCE_MEAN = 1
+LSP_MAX_F = 512          # B200GNN_LSP_MAX_F: widest student row b200gnn_lsp_student_f32 holds in registers
 
 _i32p = C.c_void_p
 _f32p = C.c_void_p
@@ -141,6 +142,9 @@ SIGNATURES = {
     "b200gnn_edge_sim_bwd_f32": (_int, [_f32p, _i64, _i32p, _i32p, _i64, _int, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_lsp_bwd_values_f32": (_int, [_f32p, _i64, _i32p, _i32p, _i64, _int, _f32p, _f32p, _i32p, _i32p, _i32p, _i32p, _i64,
                                           _f32p, _f32p, _ptr]),
+    "b200gnn_lsp_student_f32": (_int, [_f32p, _i64, _i32p, _i32p, _i32p, _i64, _i64, _f32p, _int, _i32p, _i32p, _i32p, _i32p,
+                                       _i64, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _ptr]),
+    "b200gnn_scatter_rows_scaled_f32": (_int, [_f32p, _ptr, _i64, _i64, _f32, _f32p, _i64, _f32p, _f32p, _ptr]),
     "b200gnn_gat_edge_softmax_f32": (_int, [_i32p, _i32p, _f32p, _f32p, _i64, _i64, _f32, _f32, _f32p, _ptr, _ptr]),
     "b200gnn_gat_aggregate_f32": (_int, [_i32p, _i32p, _i32p, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _i32p, _i64,
                                          _i32, _i32, _i32p, _i32p, _i64, _i64, _f32p, _ptr]),

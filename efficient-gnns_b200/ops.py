@@ -252,6 +252,39 @@ def gather_rows_act(x: torch.Tensor, idx: torch.Tensor, out: torch.Tensor, bits:
     return out
 
 
+def lsp_student(feat: torch.Tensor, src: torch.Tensor, dst: torch.Tensor, rowptr: torch.Tensor, sim_t: torch.Tensor, kernel: int,
+                pos_dst: torch.Tensor, pos_src: torch.Tensor, comb_rowptr: torch.Tensor, diag_pos: torch.Tensor,
+                sim_s: torch.Tensor, scratch: torch.Tensor, val: torch.Tensor, selfc: torch.Tensor, loss: torch.Tensor,
+                partial: torch.Tensor) -> None:
+    """The student side of the LSP loss (kld) over a dst-sorted edge list (criterion.LspPlan) and its backward matrix: sim_s,
+    the backward matrix's values val (selfc scratch) and loss[0], bit-identical to edge_sim -> lsp_segment -> lsp_bwd_values.
+    feat [n_nodes, F] with F <= lib.LSP_MAX_F; scratch [2E]."""
+    E, n_seg, n_nodes = src.numel(), rowptr.numel() - 1, comb_rowptr.numel() - 1
+    assert dst.numel() == E and sim_t.numel() == E and sim_s.numel() == E and scratch.numel() >= 2 * E
+    assert pos_dst.numel() == E and pos_src.numel() == E and diag_pos.numel() == n_nodes and feat.shape[0] >= n_nodes
+    assert val.numel() == selfc.numel() == 2 * E + n_nodes and partial.numel() >= int(lib.load().b200gnn_lsp_partials(n_seg))
+    i32 = lambda t, name: lib.dptr(t, torch.int32, name)
+    lib.check(lib.load().b200gnn_lsp_student_f32(
+        _f32(feat, "feat"), feat.shape[1], i32(src, "src"), i32(dst, "dst"), i32(rowptr, "rowptr"), n_seg, E,
+        _f32(sim_t, "sim_t"), int(kernel), i32(pos_dst, "pos_dst"), i32(pos_src, "pos_src"), i32(comb_rowptr, "comb_rowptr"),
+        i32(diag_pos, "diag_pos"), n_nodes, _f32(sim_s, "sim_s"), _f32(scratch, "scratch"), _f32(val, "val"),
+        _f32(selfc, "selfc"), _f32(loss, "loss"), _f32(partial, "partial"), lib.stream_ptr()), "lsp_student_f32")
+
+
+def scatter_rows_scaled(src: torch.Tensor, idx: torch.Tensor, scale: float, out: torch.Tensor,
+                        loss_aux: Optional[torch.Tensor] = None, loss_total: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[idx[i]] = src[i] * scale (fp32 product; idx int64); no other row of out is written.  With loss_total, also
+    loss_total[0] += loss_aux[0] * scale (fp32 product, then fp32 add)."""
+    n, K = src.shape
+    assert idx.numel() == n and out.dim() == 2 and out.shape[1] == K and out.stride(1) == 1
+    if out.dtype != torch.float32 or not out.is_cuda:
+        raise lib.B200GnnError("scatter_rows_scaled: out must be a float32 CUDA tensor")
+    lib.check(lib.load().b200gnn_scatter_rows_scaled_f32(
+        _f32(src, "src"), lib.dptr(idx, torch.int64, "idx"), n, K, float(scale), out.data_ptr(), out.stride(0),
+        _f32(loss_aux, "loss_aux"), _f32(loss_total, "loss_total"), lib.stream_ptr()), "scatter_rows_scaled_f32")
+    return out
+
+
 def bn_act_bwd(d_out, x_out, y, mean, invstd, gamma, p: float, d_y=None, d_gamma=None, d_beta=None, d_bias=None,
                partial=None, coef=None, want_dbias: bool = True):
     """Backward of x_out = dropout_p(relu(BN_train(y))). Returns (d_y, d_gamma, d_beta, d_bias)."""

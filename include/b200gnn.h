@@ -555,6 +555,28 @@ int b200gnn_lsp_bwd_values_f32(const float* feat, int64_t F, const int32_t* src,
                                const int32_t* pos_dst, const int32_t* pos_src,
                                const int32_t* comb_rowptr, const int32_t* diag_pos, int64_t n_nodes,
                                float* val, float* selfc, void* stream);
+/* The captured LSP step (csrc/loss_edge.cu; --training lpw, lpw_criterion :95-126 with criterion kld, on the train-induced
+ * edge list of gnn_kd_and_aux.py:240-243).  The teacher similarities sim_t[E] are a constant of the run: the caller forms
+ * them once with b200gnn_edge_sim_f32.
+ *   lsp_student: one launch sequence for the student side, bit-identical to b200gnn_edge_sim_f32(feat) ->
+ *     b200gnn_lsp_segment_f32(criterion 0) -> b200gnn_lsp_bwd_values_f32 on the same inputs: sim_s[E], val[2E + n_nodes]
+ *     (diagonal included; selfc is scratch of that size) and loss_out[0].  One warp per destination segment, the segment's
+ *     destination row held in registers: F (the student's width) at most B200GNN_LSP_MAX_F.  rowptr[n_seg + 1] groups the
+ *     dst-sorted edges by destination, pos_* / comb_rowptr / diag_pos are the backward matrix of lsp_bwd_values;
+ *     scratch: 2E floats; partial: b200gnn_lsp_partials(n_seg) floats.  Null pointers, E <= 0, n_seg <= 0, n_nodes <= 0,
+ *     kernel outside 0..3 and F outside (0, B200GNN_LSP_MAX_F] are refused before any launch.
+ *   scatter_rows_scaled: dst[idx[i]][k] = src[i][k] * scale (fp32 product, no FMA) for the n rows of src [n, K] (idx int64,
+ *     dst row pitch ldd); no other row of dst is touched.  With loss_total, thread 0 of the launch also forms
+ *     loss_total[0] = loss_total[0] + loss_aux[0] * scale (fp32 product, then fp32 add): with scale = beta this is the
+ *     d (beta * loss) / d out_feat rows and the beta * loss_aux term of the step's loss, as the eager path rounds them. */
+#define B200GNN_LSP_MAX_F 512
+int b200gnn_lsp_student_f32(const float* feat, int64_t F, const int32_t* src, const int32_t* dst, const int32_t* rowptr,
+                            int64_t n_seg, int64_t E, const float* sim_t, int kernel, const int32_t* pos_dst,
+                            const int32_t* pos_src, const int32_t* comb_rowptr, const int32_t* diag_pos, int64_t n_nodes,
+                            float* sim_s, float* scratch, float* val, float* selfc, float* loss_out, float* partial,
+                            void* stream);
+int b200gnn_scatter_rows_scaled_f32(const float* src, const int64_t* idx, int64_t n, int64_t K, float scale, float* dst,
+                                    int64_t ldd, const float* loss_aux, float* loss_total, void* stream);
 
 /* ------------------------------------------------------------------ *
  * Graph attention (BASELINE config 4): per-destination edge softmax and
