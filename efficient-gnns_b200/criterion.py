@@ -219,50 +219,93 @@ def at_criterion(logits, labels, feat, teacher_feat, beta=1000, _cls=None):
 
 
 # ----------------------------------------------------------------------------------------- GSP
+# Rows R of the two [R, Sp] Gram chunks of one GSP pass: together they take the InfoNCE chunk's budget (NCE_CHUNK_BYTES),
+# so the loss never holds the four S x S matrices (Grams and their gradients) the direct form needs: 1 GiB at S = 8192.
+def gsp_chunk_rows(Sp: int) -> int:
+    """Rows R of one pair of [R, Sp] Gram chunks (2 * R * Sp * 4 <= NCE_CHUNK_BYTES, a multiple of 128, at most Sp)."""
+    return min(max(128, (NCE_CHUNK_BYTES // (8 * Sp)) // 128 * 128), Sp)
+
+
+class GspBuffers:
+    """Every buffer of one GSP forward + gradient over [Sp, Fp] student and [Sp, Fp_t] teacher operands (Fp_t = Fp unless
+    given: each side only meets itself), allocated once so that a captured step (gsp.py) reuses them on every replay.
+    ns / nt [Sp]: the operands' squared row norms, filled by the caller for l2 / rbf.  g_s [Sp, Fp] / g_t [Sp, Fp_t]: dG . x
+    per side (rows < S), the operand gradient before the factor 2 and the norm terms."""
+
+    def __init__(self, Sp: int, Fp: int, device, Fp_t: Optional[int] = None):
+        R = gsp_chunk_rows(Sp)
+        Ft = Fp if Fp_t is None else Fp_t
+        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=device)
+        self.Gs, self.Gt = e(R, Sp), e(R, Sp)
+        self.xs_split, self.xt_split = (e(Sp, Fp), e(Sp, Fp)), (e(Sp, Ft), e(Sp, Ft))          # B of G_c = x_c . x^T
+        self.xsT_split, self.xtT_split = (e(Fp, Sp), e(Fp, Sp)), (e(Ft, Sp), e(Ft, Sp))      # B of g_c = dG_c . x
+        self.ns, self.nt, self.rc_s, self.rc_t, self.part = e(Sp), e(Sp), e(Sp), e(Sp), e(Sp)
+        self.loss = e(1)
+        self.g_s, self.g_t = e(Sp, Fp), e(Sp, Ft)
+
+
+def gsp_chunks(x_s: torch.Tensor, x_t: torch.Tensor, S: int, kernel: int, b: GspBuffers) -> None:
+    """The GSP loss over zero-padded operands x_s [Sp, Fp], x_t [Sp, Fp_t] (S real rows; normalised for cosine / poly, raw for l2 / rbf
+    with b.ns / b.nt holding their squared norms) in row chunks: per chunk the two Gram GEMMs x_c . x^T, the pair pass
+    (both gradients in place, the padding columns zeroed), then g[c] = dG_c . x per side.  dG is symmetric, so d x = 2 dG x
+    needs only the chunk's own rows.  b.loss = mse(sim_s, sim_t); b.rc_s / b.rc_t the l2 / rbf row coefficients.  Only
+    launches on preallocated buffers, so it can be captured."""
+    L, st = _L(), lib.stream_ptr()
+    Sp = x_s.shape[0]
+    R = b.Gs.shape[0]
+    sides = ((x_s, b.xs_split, b.xsT_split, b.Gs, b.g_s), (x_t, b.xt_split, b.xtT_split, b.Gt, b.g_t))
+    for x, sp, spT, _, _ in sides:
+        ops.split_tf32(x, hi=sp[0], lo=sp[1])
+        ops.split_tf32(x, transpose=True, hi=spT[0], lo=spT[1])
+    raw = kernel >= 2
+    for r0 in range(0, S, R):
+        r = min(R, S - r0)
+        for x, sp, _, G, _ in sides:
+            ops.gemm_tf32x3(x[r0:r0 + r], sp[0], sp[1], out=G[:r])
+        lib.check(L.b200gnn_gsp_pair_chunk_f32(_f32(b.Gs, "Gs"), _f32(b.Gt, "Gt"), Sp, r, S, r0, _f32(b.ns if raw else None, "ns"),
+                                               _f32(b.nt if raw else None, "nt"), kernel, _f32(b.rc_s if raw else None, "rc_s"),
+                                               _f32(b.rc_t if raw else None, "rc_t"), _f32(b.part, "part"), st),
+                  "gsp_pair_chunk_f32")
+        for _, _, spT, G, g in sides:
+            ops.gemm_tf32x3(G[:r], spT[0], spT[1], out=g[r0:r0 + r])
+    lib.check(L.b200gnn_gsp_finish_f32(_f32(b.part, "part"), S, _f32(b.loss, "loss"), st), "gsp_finish_f32")
+
+
 class _GSP(torch.autograd.Function):
-    """mse(pairwise_k(fs), pairwise_k(ft)) over an S-row sample (criterion.py:66-86), S x S never leaves HBM twice:
-    Gram matrices by wgmma GEMM, similarity + MSE + d/dGram in one pass per side."""
+    """mse(pairwise_k(fs), pairwise_k(ft)) over an S-row sample (criterion.py:66-86) by gsp_chunks: the S x S Gram
+    matrices exist only as L2-sized row chunks, and both gradients are complete when the forward returns."""
 
     @staticmethod
     def forward(ctx, fs, ft, kernel: int):
         fs, ft = fs.contiguous(), ft.contiguous()
         L, st = _L(), lib.stream_ptr()
-        S = fs.shape[0]
+        S, F_, F_t = fs.shape[0], fs.shape[1], ft.shape[1]
         if kernel <= 1:
             xs, ns = _normalize(fs)
             xt, nt = _normalize(ft)
-            sq_s = sq_t = None
         else:
             xs, xt, ns, nt = fs, ft, None, None
-            sq_s, sq_t = _new(S, like=fs), _new(S, like=fs)
-            lib.check(L.b200gnn_row_sqnorm_f32(_f32(xs, "xs"), S, xs.shape[1], _f32(sq_s, "sq"), st), "row_sqnorm_f32")
-            lib.check(L.b200gnn_row_sqnorm_f32(_f32(xt, "xt"), S, xt.shape[1], _f32(sq_t, "sq"), st), "row_sqnorm_f32")
-        Gs, Gt = _gemm_nt(xs, xs), _gemm_nt(xt, xt)
-        loss, part = _new(1, like=fs), _new(S, like=fs)
-        dGs, dGt = Gs.clone(), Gt.clone()
-        rc_s = _new(S, like=fs) if kernel >= 2 else None
-        rc_t = _new(S, like=fs) if kernel >= 2 else None
-        lib.check(L.b200gnn_gsp_pair_f32(_f32(dGs, "Gs"), _f32(Gt, "Gt"), _f32(sq_s, "ns"), _f32(sq_t, "nt"), S, kernel,
-                                         _f32(rc_s, "rc"), _f32(loss, "loss"), _f32(part, "part"), st), "gsp_pair_f32")
-        loss2 = _new(1, like=fs)
-        lib.check(L.b200gnn_gsp_pair_f32(_f32(dGt, "Gt"), _f32(Gs, "Gs"), _f32(sq_t, "nt"), _f32(sq_s, "ns"), S, kernel,
-                                         _f32(rc_t, "rc"), _f32(loss2, "loss"), _f32(part, "part"), st), "gsp_pair_f32")
+        xs_p, xt_p = _pad_k(_pad_k(xs, 1), 0), _pad_k(_pad_k(xt, 1), 0)
+        b = GspBuffers(xs_p.shape[0], xs_p.shape[1], fs.device, xt_p.shape[1])
+        if kernel >= 2:
+            lib.check(L.b200gnn_row_sqnorm_f32(_f32(xs, "xs"), S, F_, _f32(b.ns, "sq"), st), "row_sqnorm_f32")
+            lib.check(L.b200gnn_row_sqnorm_f32(_f32(xt, "xt"), S, F_t, _f32(b.nt, "sq"), st), "row_sqnorm_f32")
+        gsp_chunks(xs_p, xt_p, S, kernel, b)
         ctx.kernel = kernel
-        ctx.save_for_backward(xs, xt, ns if ns is not None else xs, nt if nt is not None else xt, dGs, dGt,
-                              rc_s if rc_s is not None else xs, rc_t if rc_t is not None else xt)
-        return loss[0]
+        ctx.save_for_backward(xs, xt, ns if ns is not None else xs, nt if nt is not None else xt, b.g_s[:S, :F_], b.g_t[:S, :F_t],
+                              b.rc_s[:S], b.rc_t[:S])
+        return b.loss[0]
 
     @staticmethod
     def backward(ctx, g):
-        xs, xt, ns, nt, dGs, dGt, rc_s, rc_t = ctx.saved_tensors
+        xs, xt, ns, nt, g_s, g_t, rc_s, rc_t = ctx.saved_tensors
         L, st = _L(), lib.stream_ptr()
         out = []
-        for x, nrm, dG, rc, need in ((xs, ns, dGs, rc_s, ctx.needs_input_grad[0]), (xt, nt, dGt, rc_t, ctx.needs_input_grad[1])):
+        for x, nrm, dGx, rc, need in ((xs, ns, g_s, rc_s, ctx.needs_input_grad[0]), (xt, nt, g_t, rc_t, ctx.needs_input_grad[1])):
             if not need:
                 out.append(None)
                 continue
-            d = _gemm_nn(dG, x)                     # dG @ x  ;  d x = 2 dG x (+ norm terms)
-            d.mul_(2.0)
+            d = (dGx * 2.0).contiguous()            # d x = 2 dG x (+ norm terms)
             if ctx.kernel >= 2:
                 lib.check(L.b200gnn_row_axpy_f32(_f32(x, "x"), _f32(rc, "rc"), x.shape[0], x.shape[1], 4.0, _f32(d, "d"), st),
                           "row_axpy_f32")

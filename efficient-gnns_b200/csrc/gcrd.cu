@@ -6,6 +6,10 @@
 // Head h (s = student, t = teacher) over the n_train training rows: pre_h = G_h W_h^T + b_h (row pitch P), bn_h = [4][P]
 // (mean, invstd, scale, shift of b200gnn_bn_finalize_f32), P_h = relu(pre_h * scale + shift).  Sampled position j is
 // training row inds[j]; x_h[j] = scale_h * P_h[inds[j]] / max(||P_h[inds[j]]||, eps) (scale_s = 1 / nce_T, scale_t = 1).
+//
+// GSP (global structure preservation, arxiv_pyg/criterion.py:57-92) on the same heads uses the same two row passes:
+// cosine / poly take the normalising path with scale 1 on both sides; l2 / rbf the raw path, x_h[j] = P_h[inds[j]] with
+// its squared norm, and on the way back the norm term of the distance instead of the normalise backward.
 #include "common.cuh"
 #include "philox.cuh"
 
@@ -38,6 +42,8 @@ __global__ void __launch_bounds__(256) sample_keys_kernel(int64_t n, uint64_t se
 }
 
 // One head's operand row: x = sc * relu(bn(pre)) / max(||.||, eps), norm = ||relu(bn(pre))||.
+// RAW: x = relu(bn(pre)), norm = its squared norm (sc and eps unused).
+template <bool RAW>
 __device__ __forceinline__ void operand_row(const float* __restrict__ pre, const float* __restrict__ bn, int P, float sc, float eps,
                                             float* __restrict__ x, float* __restrict__ norm, int lane) {
   float4 a[2];
@@ -55,15 +61,25 @@ __device__ __forceinline__ void operand_row(const float* __restrict__ pre, const
     }
   }
   ss = warp_sum(ss);
-  const float nrm = sqrtf(ss), inv = sc / fmaxf(nrm, eps);
+  if constexpr (RAW) {
 #pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const int c4 = 4 * (lane + 32 * k);
-    if (c4 < P) st4(x + c4, make_float4(a[k].x * inv, a[k].y * inv, a[k].z * inv, a[k].w * inv));
+    for (int k = 0; k < 2; ++k) {
+      const int c4 = 4 * (lane + 32 * k);
+      if (c4 < P) st4(x + c4, a[k]);
+    }
+    if (lane == 0) *norm = ss;
+  } else {
+    const float nrm = sqrtf(ss), inv = sc / fmaxf(nrm, eps);
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int c4 = 4 * (lane + 32 * k);
+      if (c4 < P) st4(x + c4, make_float4(a[k].x * inv, a[k].y * inv, a[k].z * inv, a[k].w * inv));
+    }
+    if (lane == 0) *norm = nrm;
   }
-  if (lane == 0) *norm = nrm;
 }
 
+template <bool RAW>
 __global__ void __launch_bounds__(256) operands_kernel(const int32_t* __restrict__ inds, int64_t S, int P,
                                                        const float* __restrict__ pre_s, const float* __restrict__ bn_s,
                                                        const float* __restrict__ pre_t, const float* __restrict__ bn_t, float inv_T,
@@ -72,18 +88,24 @@ __global__ void __launch_bounds__(256) operands_kernel(const int32_t* __restrict
   const int lane = threadIdx.x & 31;
   for (int64_t j = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); j < S; j += (int64_t)gridDim.x * 8) {
     const int64_t r = __ldg(inds + j);
-    operand_row(pre_s + r * P, bn_s, P, inv_T, eps, x_s + j * P, norm_s + j, lane);
-    operand_row(pre_t + r * P, bn_t, P, 1.f, eps, x_t + j * P, norm_t + j, lane);
+    operand_row<RAW>(pre_s + r * P, bn_s, P, inv_T, eps, x_s + j * P, norm_s + j, lane);
+    operand_row<RAW>(pre_t + r * P, bn_t, P, 1.f, eps, x_t + j * P, norm_t + j, lane);
   }
 }
 
-// One head's way back over the sampled rows of warp gw: normalise backward (the row_normalize_bwd_kernel formula), the ReLU
-// mask relu(bn(pre)) > 0, times beta -> dz stored to row inds[j] of the zero-filled [n_train, P] dz; the warp's column sums
-// of dz and dz * xhat (pass 1 of the BatchNorm backward) go to part[gw][2][P].
+// What g holds on the way back: the InfoNCE operand gradient itself (G-CRD), or dG . x of the GSP chunk loop, whose
+// operand gradient is 2 dG . x (normalising path) or 2 dG . x + 4 rc[j] x (raw path: the distance's norm terms).
+enum BwdMode { BWD_NCE = 0, BWD_GSP_NORM = 1, BWD_GSP_RAW = 2 };
+
+// One head's way back over the sampled rows of warp gw: the operand gradient, normalise backward (the
+// row_normalize_bwd_kernel formula; none on the raw path), the ReLU mask relu(bn(pre)) > 0, times beta -> dz stored to row
+// inds[j] of the zero-filled [n_train, P] dz; the warp's column sums of dz and dz * xhat (pass 1 of the BatchNorm backward)
+// go to part[gw][2][P].
+template <int MODE>
 __device__ __forceinline__ void head_bwd(int gw, int nw, int lane, const int32_t* __restrict__ inds, int64_t S, int P,
                                          const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ nrm_in,
-                                         float sc, float eps, const float* __restrict__ pre, const float* __restrict__ bn, float beta,
-                                         float* __restrict__ dz, float* __restrict__ part) {
+                                         const float* __restrict__ rc, float sc, float eps, const float* __restrict__ pre,
+                                         const float* __restrict__ bn, float beta, float* __restrict__ dz, float* __restrict__ part) {
   const float inv_sc = 1.f / sc;
   float4 s[2], q[2], mu[2], is[2], scl[2], shf[2];
 #pragma unroll
@@ -102,14 +124,23 @@ __device__ __forceinline__ void head_bwd(int gw, int nw, int lane, const int32_t
       gv[k] = xv[k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (c4 < P) {
         gv[k] = ld4(g + j * P + c4); xv[k] = ld4(x + j * P + c4);
-        dot = fmaf(xv[k].x * inv_sc, gv[k].x, dot); dot = fmaf(xv[k].y * inv_sc, gv[k].y, dot);
-        dot = fmaf(xv[k].z * inv_sc, gv[k].z, dot); dot = fmaf(xv[k].w * inv_sc, gv[k].w, dot);
+        if constexpr (MODE != BWD_NCE) { gv[k].x *= 2.f; gv[k].y *= 2.f; gv[k].z *= 2.f; gv[k].w *= 2.f; }
+        if constexpr (MODE != BWD_GSP_RAW) {
+          dot = fmaf(xv[k].x * inv_sc, gv[k].x, dot); dot = fmaf(xv[k].y * inv_sc, gv[k].y, dot);
+          dot = fmaf(xv[k].z * inv_sc, gv[k].z, dot); dot = fmaf(xv[k].w * inv_sc, gv[k].w, dot);
+        }
       }
     }
-    dot = warp_sum(dot);
-    const float nr = __ldg(nrm_in + j);
-    const bool clamped = nr < eps;
-    const float inv = sc / fmaxf(nr, eps);
+    float inv = 0.f, rcj = 0.f;
+    bool clamped = false;
+    if constexpr (MODE == BWD_GSP_RAW) {
+      rcj = 4.f * __ldg(rc + j);
+    } else {
+      dot = warp_sum(dot);
+      const float nr = __ldg(nrm_in + j);
+      clamped = nr < eps;
+      inv = sc / fmaxf(nr, eps);
+    }
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       const int c4 = 4 * (lane + 32 * k);
@@ -122,7 +153,9 @@ __device__ __forceinline__ void head_bwd(int gw, int nw, int lane, const int32_t
       float ps[4] = {0.f, 0.f, 0.f, 0.f}, pq[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float v = clamped ? d[e] * inv : inv * (d[e] - xs[e] * inv_sc * dot);
+        float v;
+        if constexpr (MODE == BWD_GSP_RAW) v = fmaf(rcj, xs[e], d[e]);
+        else v = clamped ? d[e] * inv : inv * (d[e] - xs[e] * inv_sc * dot);
         d[e] = fmaf(ys[e], a4[e], b4[e]) > 0.f ? v * beta : 0.f;
         ps[e] = d[e];
         pq[e] = d[e] * ((ys[e] - m4[e]) * i4[e]);
@@ -139,18 +172,20 @@ __device__ __forceinline__ void head_bwd(int gw, int nw, int lane, const int32_t
   }
 }
 
+template <int MODE>
 __global__ void __launch_bounds__(256) backward_kernel(const int32_t* __restrict__ inds, int64_t S, int P, const float* __restrict__ g_s,
                                                        const float* __restrict__ g_t, const float* __restrict__ x_s,
                                                        const float* __restrict__ x_t, const float* __restrict__ norm_s,
-                                                       const float* __restrict__ norm_t, float inv_T, float eps,
+                                                       const float* __restrict__ norm_t, const float* __restrict__ rc_s,
+                                                       const float* __restrict__ rc_t, float inv_T, float eps,
                                                        const float* __restrict__ pre_s, const float* __restrict__ bn_s,
                                                        const float* __restrict__ pre_t, const float* __restrict__ bn_t, float beta,
                                                        float* __restrict__ dz_s, float* __restrict__ dz_t, float* __restrict__ part_s,
                                                        float* __restrict__ part_t, const float* __restrict__ loss_aux,
                                                        float* __restrict__ loss_total) {
   const int lane = threadIdx.x & 31, gw = blockIdx.x * 8 + (threadIdx.x >> 5), nw = gridDim.x * 8;
-  head_bwd(gw, nw, lane, inds, S, P, g_s, x_s, norm_s, inv_T, eps, pre_s, bn_s, beta, dz_s, part_s);
-  head_bwd(gw, nw, lane, inds, S, P, g_t, x_t, norm_t, 1.f, eps, pre_t, bn_t, beta, dz_t, part_t);
+  head_bwd<MODE>(gw, nw, lane, inds, S, P, g_s, x_s, norm_s, rc_s, inv_T, eps, pre_s, bn_s, beta, dz_s, part_s);
+  head_bwd<MODE>(gw, nw, lane, inds, S, P, g_t, x_t, norm_t, rc_t, 1.f, eps, pre_t, bn_t, beta, dz_t, part_t);
   if (loss_total && blockIdx.x == 0 && threadIdx.x == 0) loss_total[0] += beta * loss_aux[0];
 }
 
@@ -194,8 +229,8 @@ extern "C" int b200gnn_gcrd_operands_f32(const int32_t* inds, int64_t S, int64_t
     return B200GNN_ERR_BAD_ARG;
   int64_t g = (S + 7) / 8;
   if (g > 132 * 8) g = 132 * 8;
-  gcrd::operands_kernel<<<(int)g, 256, 0, (cudaStream_t)stream>>>(inds, S, (int)P, pre_s, bn_s, pre_t, bn_t, inv_T, eps, x_s, x_t,
-                                                                  norm_s, norm_t);
+  gcrd::operands_kernel<false><<<(int)g, 256, 0, (cudaStream_t)stream>>>(inds, S, (int)P, pre_s, bn_s, pre_t, bn_t, inv_T, eps, x_s,
+                                                                         x_t, norm_s, norm_t);
   return check_launch();
 }
 
@@ -212,8 +247,52 @@ extern "C" int b200gnn_gcrd_backward_f32(const int32_t* inds, int64_t S, int64_t
   const void* v4[] = {g_s, g_t, x_s, x_t, pre_s, pre_t, bn_s, bn_t, dz_s, dz_t, part_s, part_t};
   for (const void* p : v4)
     if (!aligned_to(p, 16)) return B200GNN_ERR_BAD_ARG;
-  gcrd::backward_kernel<<<gcrd::BWD_CTAS, 256, 0, (cudaStream_t)stream>>>(inds, S, (int)P, g_s, g_t, x_s, x_t, norm_s, norm_t, inv_T,
-                                                                          eps, pre_s, bn_s, pre_t, bn_t, beta, dz_s, dz_t, part_s,
-                                                                          part_t, loss_aux, loss_total);
+  gcrd::backward_kernel<gcrd::BWD_NCE><<<gcrd::BWD_CTAS, 256, 0, (cudaStream_t)stream>>>(
+      inds, S, (int)P, g_s, g_t, x_s, x_t, norm_s, norm_t, nullptr, nullptr, inv_T, eps, pre_s, bn_s, pre_t, bn_t, beta, dz_s, dz_t,
+      part_s, part_t, loss_aux, loss_total);
+  return check_launch();
+}
+
+// GSP over the same heads (kernel 0 cosine, 1 poly: normalising path, scale 1; 2 l2, 3 rbf: raw path).
+extern "C" int b200gnn_gsp_operands_f32(const int32_t* inds, int64_t S, int64_t P, int kernel, const float* pre_s, const float* bn_s,
+                                        const float* pre_t, const float* bn_t, float eps, float* x_s, float* x_t, float* norm_s,
+                                        float* norm_t, void* stream) {
+  if (!inds || S < 1 || P < 4 || P % 4 || P > gcrd::MAX_P || kernel < 0 || kernel > 3 || !pre_s || !bn_s || !pre_t || !bn_t ||
+      !x_s || !x_t || !norm_s || !norm_t || !(eps > 0.f))
+    return B200GNN_ERR_BAD_ARG;
+  const void* v4[] = {pre_s, pre_t, bn_s, bn_t, x_s, x_t};
+  for (const void* p : v4)
+    if (!aligned_to(p, 16)) return B200GNN_ERR_BAD_ARG;
+  int64_t g = (S + 7) / 8;
+  if (g > 132 * 8) g = 132 * 8;
+  if (kernel >= 2)
+    gcrd::operands_kernel<true><<<(int)g, 256, 0, (cudaStream_t)stream>>>(inds, S, (int)P, pre_s, bn_s, pre_t, bn_t, 1.f, eps, x_s, x_t,
+                                                                          norm_s, norm_t);
+  else
+    gcrd::operands_kernel<false><<<(int)g, 256, 0, (cudaStream_t)stream>>>(inds, S, (int)P, pre_s, bn_s, pre_t, bn_t, 1.f, eps, x_s,
+                                                                           x_t, norm_s, norm_t);
+  return check_launch();
+}
+
+extern "C" int b200gnn_gsp_backward_f32(const int32_t* inds, int64_t S, int64_t P, int kernel, const float* g_s, const float* g_t,
+                                        const float* x_s, const float* x_t, const float* norm_s, const float* norm_t,
+                                        const float* rc_s, const float* rc_t, float eps, const float* pre_s, const float* bn_s,
+                                        const float* pre_t, const float* bn_t, float beta, float* dz_s, float* dz_t, float* part_s,
+                                        float* part_t, const float* loss_aux, float* loss_total, void* stream) {
+  if (!inds || S < 1 || P < 4 || P % 4 || P > gcrd::MAX_P || kernel < 0 || kernel > 3 || !g_s || !g_t || !x_s || !x_t || !pre_s ||
+      !bn_s || !pre_t || !bn_t || !dz_s || !dz_t || !part_s || !part_t || !(eps > 0.f) || (loss_total && !loss_aux))
+    return B200GNN_ERR_BAD_ARG;
+  if (kernel >= 2 ? (!rc_s || !rc_t) : (!norm_s || !norm_t)) return B200GNN_ERR_BAD_ARG;
+  const void* v4[] = {g_s, g_t, x_s, x_t, pre_s, pre_t, bn_s, bn_t, dz_s, dz_t, part_s, part_t};
+  for (const void* p : v4)
+    if (!aligned_to(p, 16)) return B200GNN_ERR_BAD_ARG;
+  if (kernel >= 2)
+    gcrd::backward_kernel<gcrd::BWD_GSP_RAW><<<gcrd::BWD_CTAS, 256, 0, (cudaStream_t)stream>>>(
+        inds, S, (int)P, g_s, g_t, x_s, x_t, norm_s, norm_t, rc_s, rc_t, 1.f, eps, pre_s, bn_s, pre_t, bn_t, beta, dz_s, dz_t,
+        part_s, part_t, loss_aux, loss_total);
+  else
+    gcrd::backward_kernel<gcrd::BWD_GSP_NORM><<<gcrd::BWD_CTAS, 256, 0, (cudaStream_t)stream>>>(
+        inds, S, (int)P, g_s, g_t, x_s, x_t, norm_s, norm_t, rc_s, rc_t, 1.f, eps, pre_s, bn_s, pre_t, bn_t, beta, dz_s, dz_t,
+        part_s, part_t, loss_aux, loss_total);
   return check_launch();
 }

@@ -162,50 +162,76 @@ __global__ void __launch_bounds__(256) transpose_kernel(const float* __restrict_
 // Gs = fs fs^T, Gt = ft ft^T  (S x S Gram matrices from the GEMM; for cosine/poly the operands were normalised).
 // kernel: 0 cosine  sim = G ; 1 poly  sim = G^2 ; 2 l2  sim = sqrt(max(ni + nj - 2G, 0)) ; 3 rbf  sim = exp(-0.5 (ni+nj-2G))
 // loss = mean (sim_s - sim_t)^2 ;  Gs <- d loss / d Gs  (so that  d fs = (dG + dG^T) fs = 2 dG fs, dG symmetric),
-// and for l2/rbf rowcoef[i] += sum_j d loss/d(ni)  (the norm terms of the distance).
-__global__ void __launch_bounds__(256) gsp_pair_kernel(float* __restrict__ Gs, const float* __restrict__ Gt,
-                                                       const float* __restrict__ ns, const float* __restrict__ nt, int S,
-                                                       int kernel, float w /* 2 / S^2 */, float* __restrict__ rowcoef,
-                                                       float* __restrict__ partial) {
+// and for l2/rbf rc_s[i] = sum_j d loss/d(ni)  (the norm terms of the distance).
+// Row-chunk form: Gs / Gt hold rows [row0, row0 + gridDim.x) of the two S x S matrices at row pitch ld >= S; the l2/rbf
+// diagonal and the ns[i] / nt[i] lookups use the global row, partial[] and rc_*[] are stored at it, and columns S..ld-1
+// are set to zero (so a GEMM may contract over the padded pitch).  BOTH: Gt <- d loss / d Gt in the same pass, with the
+// teacher's own coefficient sums in rc_t; its expressions are the student's with the roles of the two sides swapped, so
+// the result is that of a second one-sided pass on (Gt, Gs, nt, ns).
+template <bool BOTH>
+__global__ void __launch_bounds__(256) gsp_pair_kernel(float* __restrict__ Gs, float* __restrict__ Gt, int64_t ld, int S,
+                                                       int row0, const float* __restrict__ ns, const float* __restrict__ nt,
+                                                       int kernel, float w /* 2 / S^2 */, float* __restrict__ rc_s,
+                                                       float* __restrict__ rc_t, float* __restrict__ partial) {
   __shared__ float s_red[32];
-  const int row = blockIdx.x;
-  float* gs = Gs + (size_t)row * S;
-  const float* gt = Gt + (size_t)row * S;
-  float acc = 0.f, rc = 0.f;
+  const int row = row0 + blockIdx.x;
+  float* gs = Gs + (size_t)blockIdx.x * ld;
+  float* gt = Gt + (size_t)blockIdx.x * ld;
+  float acc = 0.f, rs = 0.f, rt = 0.f;
   const float nsi = (kernel >= 2) ? ns[row] : 0.f, nti = (kernel >= 2) ? nt[row] : 0.f;
   for (int j = threadIdx.x; j < S; j += blockDim.x) {
-    float ss, st, dsim_dg, dsim_dn = 0.f;   // d sim_s / d Gs_ij , d sim_s / d ns_i (= d/d ns_j)
+    float ss, st, ds_dg, dt_dg, ds_dn = 0.f, dt_dn = 0.f;   // d sim / d G_ij , d sim / d n_i (= d/d n_j), per side
     const float a = gs[j], b = gt[j];
-    if (kernel == 0) { ss = a; st = b; dsim_dg = 1.f; }
-    else if (kernel == 1) { ss = a * a; st = b * b; dsim_dg = 2.f * a; }
+    if (kernel == 0) { ss = a; st = b; ds_dg = 1.f; dt_dg = 1.f; }
+    else if (kernel == 1) { ss = a * a; st = b * b; ds_dg = 2.f * a; dt_dg = 2.f * b; }
     else {
       float d2s = fmaxf(nsi + ns[j] - 2.f * a, 0.f), d2t = fmaxf(nti + nt[j] - 2.f * b, 0.f);
       if (j == row) { d2s = 0.f; d2t = 0.f; }
       if (kernel == 2) {
         ss = sqrtf(d2s); st = sqrtf(d2t);
-        const float inv = ss > 0.f ? 0.5f / ss : 0.f;     // d sqrt(d2)/d d2, sub-gradient 0 at 0 (torch .norm backward)
-        dsim_dg = -2.f * inv; dsim_dn = inv;
+        const float inv_s = ss > 0.f ? 0.5f / ss : 0.f;   // d sqrt(d2)/d d2, sub-gradient 0 at 0 (torch .norm backward)
+        const float inv_t = st > 0.f ? 0.5f / st : 0.f;
+        ds_dg = -2.f * inv_s; ds_dn = inv_s;
+        dt_dg = -2.f * inv_t; dt_dn = inv_t;
       } else {
         ss = expf(-0.5f * d2s); st = expf(-0.5f * d2t);
-        dsim_dg = ss; dsim_dn = -0.5f * ss;
+        ds_dg = ss; ds_dn = -0.5f * ss;
+        dt_dg = st; dt_dn = -0.5f * st;
       }
     }
     const float diff = ss - st;
     acc = fmaf(diff, diff, acc);
     const float g = w * diff;                 // d loss / d sim_s
-    gs[j] = g * dsim_dg;
-    rc += g * dsim_dn;
+    gs[j] = g * ds_dg;
+    rs += g * ds_dn;
+    if (BOTH) {
+      const float diff_t = st - ss;
+      const float g_t = w * diff_t;           // d loss / d sim_t
+      gt[j] = g_t * dt_dg;
+      rt += g_t * dt_dn;
+    }
+  }
+  for (int64_t j = (int64_t)S + threadIdx.x; j < ld; j += blockDim.x) {
+    gs[j] = 0.f;
+    if (BOTH) gt[j] = 0.f;
   }
   // block reductions (deterministic)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  acc = warp_sum_f(acc); rc = warp_sum_f(rc);
+  acc = warp_sum_f(acc); rs = warp_sum_f(rs);
+  if (BOTH) rt = warp_sum_f(rt);
   if (lane == 0) s_red[warp] = acc;
   __syncthreads();
   if (warp == 0) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) partial[row] = t; }
   __syncthreads();
-  if (lane == 0) s_red[warp] = rc;
+  if (lane == 0) s_red[warp] = rs;
   __syncthreads();
-  if (warp == 0 && rowcoef) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) rowcoef[row] = t; }
+  if (warp == 0 && rc_s) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) rc_s[row] = t; }
+  if (BOTH) {
+    __syncthreads();
+    if (lane == 0) s_red[warp] = rt;
+    __syncthreads();
+    if (warp == 0 && rc_t) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) rc_t[row] = t; }
+  }
 }
 
 // d fs[i,:] += coef[i] * fs[i,:]     (norm terms of l2 / rbf:  d n_i / d fs_i = 2 fs_i, coefficient folded by the caller)
@@ -355,9 +381,36 @@ extern "C" int b200gnn_gsp_pair_f32(float* Gs, const float* Gt, const float* ns,
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
   const double n2 = (double)S * (double)S;
-  gsp_pair_kernel<<<(int)S, 256, 0, st>>>(Gs, Gt, ns, nt, (int)S, kernel, (float)(2.0 / n2), rowcoef, partial);
+  // the one-sided pass never stores to Gt
+  gsp_pair_kernel<false><<<(int)S, 256, 0, st>>>(Gs, const_cast<float*>(Gt), S, (int)S, 0, ns, nt, kernel, (float)(2.0 / n2),
+                                                 rowcoef, nullptr, partial);
   if ((rc = check_launch())) return rc;
   sum_partials_kernel<<<1, 256, 0, st>>>(partial, (int)S, 1.0 / n2, loss_out);
+  return check_launch();
+}
+
+// Both gradients of a row chunk in one pass: Gs / Gt rows [row_offset, row_offset + n_rows) of the two S x S Gram
+// matrices (row pitch ld >= S, a multiple of 4 when a GEMM reads them back), overwritten by d loss / d Gs and d loss / d Gt;
+// columns S..ld-1 are set to zero.  partial[S] and (l2 / rbf) rc_s[S] / rc_t[S] are stored at the global rows, so
+// b200gnn_gsp_finish_f32 gives the same loss bits for any chunking.
+extern "C" int b200gnn_gsp_pair_chunk_f32(float* Gs, float* Gt, int64_t ld, int64_t n_rows, int64_t S, int64_t row_offset,
+                                          const float* ns, const float* nt, int kernel, float* rc_s, float* rc_t, float* partial,
+                                          void* stream) {
+  if (!Gs || !Gt || !partial || S <= 0 || S >= INT32_MAX || ld < S || n_rows <= 0 || row_offset < 0 ||
+      row_offset + n_rows > S || kernel < 0 || kernel > 3)
+    return B200GNN_ERR_BAD_ARG;
+  if (kernel >= 2 && (!ns || !nt || !rc_s || !rc_t)) return B200GNN_ERR_BAD_ARG;
+  const double n2 = (double)S * (double)S;
+  gsp_pair_kernel<true><<<(int)n_rows, 256, 0, (cudaStream_t)stream>>>(Gs, Gt, ld, (int)S, (int)row_offset, ns, nt, kernel,
+                                                                      (float)(2.0 / n2), rc_s, rc_t, partial);
+  return check_launch();
+}
+
+// loss_out[0] = sum(partial[0..S)) / S^2: the GSP loss from the chunk passes' partials.
+extern "C" int b200gnn_gsp_finish_f32(const float* partial, int64_t S, float* loss_out, void* stream) {
+  if (!partial || !loss_out || S <= 0 || S >= INT32_MAX) return B200GNN_ERR_BAD_ARG;
+  const double n2 = (double)S * (double)S;
+  sum_partials_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(partial, (int)S, 1.0 / n2, loss_out);
   return check_launch();
 }
 

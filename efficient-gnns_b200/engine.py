@@ -54,12 +54,15 @@ class GCNStudentTrainer:
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
                  aggregate_first: Optional[bool] = None, tensor_core_gemm: bool = True, overlap_wgrad: bool = True,
                  fuse_row_passes: bool = True, fuse_activations: bool = True, _prebuilt_graph: Optional[CsrGraph] = None, _rows_alloc: Optional[int] = None,
-                 gcrd=None, lsp=None):
+                 gcrd=None, lsp=None, gsp=None):
         """gcrd: a gcrd.GCRD whose projection heads and InfoNCE loss run inside this trainer's step (kd or supervised + beta *
-        G-CRD, one CUDA graph); lsp: an lsp.LSP run the same way (kd or supervised + beta * LSP); None for both leaves the step
-        as it is."""
+        G-CRD, one CUDA graph); lsp: an lsp.LSP run the same way (kd or supervised + beta * LSP); gsp: a gsp.GSP, the
+        projection heads of G-CRD with the pairwise-similarity loss (kd or supervised + beta * GSP); at most one of the three,
+        and None for all leaves the step as it is."""
         if gcrd is not None and lsp is not None:
             raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
+        if gsp is not None and (gcrd is not None or lsp is not None):
+            raise ValueError("gsp= and the gcrd= / lsp= objective are two auxiliary losses; pass one")
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         self.device = adj.device
         self.dims, self.L = list(dims), len(dims) - 1
@@ -184,7 +187,8 @@ class GCNStudentTrainer:
         self._static: Dict[str, torch.Tensor] = {}
         for k in set(dims[1:]):
             self._part(k); self._coef(k)
-        self.objective = gcrd if gcrd is not None else lsp      # the auxiliary loss run inside the step, if any
+        # the auxiliary loss run inside the step, if any
+        self.objective = next((o for o in (gcrd, lsp, gsp) if o is not None), None)
         if self.objective is not None:
             self.objective.bind(self)
 
@@ -440,8 +444,8 @@ class GCNStudentTrainer:
         ``lambda f: criterion.lpw_criterion(z, y, f[idx], t_feat[idx], edge_index, "cosine", 1)[2]`` or a projection head +
         ``nce_criterion``; parameters of such heads get their gradients through torch autograd and stay with the caller's
         optimizer.  Returns the device tensor [loss, loss_cls, loss_kd] (+ beta*aux folded into loss); no host sync.
-        With a G-CRD or LSP object (constructor) the step includes it (loss[0] += beta * loss_aux, value in its loss_aux);
-        ``sample`` (positions into train_idx, [S]) then replaces G-CRD's on-device row draw."""
+        With a G-CRD, LSP or GSP object (constructor) the step includes it (loss[0] += beta * loss_aux, value in its loss_aux);
+        ``sample`` (positions into train_idx, [S]) then replaces the G-CRD / GSP on-device row draw."""
         if sample is not None and self.objective is None:
             raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
         if aux is None:

@@ -31,11 +31,13 @@ from .sparse import CsrGraph, SparseTensor
 class SAGEStudentTrainer:
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
-                 fuse_row_passes: bool = True, gcrd=None, lsp=None):
-        """gcrd / lsp: a gcrd.GCRD or an lsp.LSP run inside the step as engine.GCNStudentTrainer runs it; None for both
-        leaves the step as it is."""
+                 fuse_row_passes: bool = True, gcrd=None, lsp=None, gsp=None):
+        """gcrd / lsp / gsp: a gcrd.GCRD, an lsp.LSP or a gsp.GSP run inside the step as engine.GCNStudentTrainer runs it;
+        at most one, and None for all leaves the step as it is."""
         if gcrd is not None and lsp is not None:
             raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
+        if gsp is not None and (gcrd is not None or lsp is not None):
+            raise ValueError("gsp= and the gcrd= / lsp= objective are two auxiliary losses; pass one")
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         for d in dims:
             assert d % 4 == 0 and d <= 1024, "layer widths must be multiples of 4 (128-bit rows)"
@@ -99,7 +101,8 @@ class SAGEStudentTrainer:
         self.loss_aux = None
         self._graph = None
         self.reset_parameters(seed)
-        self.objective = gcrd if gcrd is not None else lsp      # the auxiliary loss run inside the step, if any
+        # the auxiliary loss run inside the step, if any
+        self.objective = next((o for o in (gcrd, lsp, gsp) if o is not None), None)
         if self.objective is not None:
             self.objective.bind(self)
 
@@ -257,8 +260,8 @@ class SAGEStudentTrainer:
     def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
                    sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One reference ``train()`` call for ``--gnn sage``: supervised / kd, or kd + beta*aux with ``aux(out_feat)`` as in
-        engine.GCNStudentTrainer.train_step, or with the G-CRD or LSP object of the constructor (``sample`` as there).  Returns
-        the device tensor [loss, loss_cls, loss_kd]."""
+        engine.GCNStudentTrainer.train_step, or with the G-CRD, LSP or GSP object of the constructor (``sample`` as there).
+        Returns the device tensor [loss, loss_cls, loss_kd]."""
         if sample is not None and self.objective is None:
             raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
         if aux is None:

@@ -135,6 +135,12 @@ SIGNATURES = {
                                          _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_transpose_f32": (_int, [_f32p, _i64, _i64, _f32p, _ptr]),
     "b200gnn_gsp_pair_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _int, _f32p, _f32p, _f32p, _ptr]),
+    "b200gnn_gsp_pair_chunk_f32": (_int, [_f32p, _f32p, _i64, _i64, _i64, _i64, _f32p, _f32p, _int, _f32p, _f32p, _f32p, _ptr]),
+    "b200gnn_gsp_finish_f32": (_int, [_f32p, _i64, _f32p, _ptr]),
+    "b200gnn_gsp_operands_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p,
+                                        _ptr]),
+    "b200gnn_gsp_backward_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32,
+                                        _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_row_axpy_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32, _f32p, _ptr]),
     "b200gnn_edge_sim_f32": (_int, [_f32p, _i64, _i32p, _i32p, _i64, _int, _f32p, _ptr]),
     "b200gnn_lsp_partials": (_i64, [_i64]),

@@ -520,6 +520,29 @@ int b200gnn_transpose_f32(const float* in, int64_t rows, int64_t cols, float* ou
 int b200gnn_gsp_pair_f32(float* Gs, const float* Gt, const float* ns, const float* nt,
                          int64_t S, int kernel, float* rowcoef, float* loss_out,
                          float* partial, void* stream);
+/* The chunked GSP pass: Gs / Gt = rows [row_offset, row_offset + n_rows) of the two S x S Gram matrices at row pitch
+ * ld >= S, overwritten in one pass by d loss / d Gs and d loss / d Gt (each equal to what b200gnn_gsp_pair_f32 stores for
+ * its side: (Gs, Gt, ns, nt) for the student, (Gt, Gs, nt, ns) for the teacher), columns S..ld-1 set to zero.  The l2 / rbf
+ * diagonal and ns / nt are taken at the global row; partial[S] and (kernels 2,3) rc_s[S] / rc_t[S] are stored there, so
+ * b200gnn_gsp_finish_f32 (loss_out[0] = sum partial / S^2) gives the same loss for any chunking. */
+int b200gnn_gsp_pair_chunk_f32(float* Gs, float* Gt, int64_t ld, int64_t n_rows, int64_t S, int64_t row_offset,
+                               const float* ns, const float* nt, int kernel, float* rc_s, float* rc_t, float* partial,
+                               void* stream);
+int b200gnn_gsp_finish_f32(const float* partial, int64_t S, float* loss_out, void* stream);
+/* The captured GSP step (csrc/gcrd.cu; gpw_criterion :57-92 on the projection heads of the G-CRD step).
+ *   gsp_operands: kernel 0 cosine / 1 poly: x_*[j] = relu(bn_*(pre_*[inds[j]])) normalised (F.normalize, eps), its norm to
+ *     norm_*[j]; kernel 2 l2 / 3 rbf: x_*[j] = relu(bn_*(pre_*[inds[j]])) and its squared norm to norm_*[j].
+ *   gsp_backward: g_* = dG_* . x_* ([S, P], the chunk loop's product); the operand gradient is 2 g (kernels 0,1, then the
+ *     normalise backward; norm_* required) or 2 g + 4 rc_*[j] x (kernels 2,3; rc_* required), then the ReLU mask, beta, dz_* and
+ *     part_* as b200gnn_gcrd_backward_f32 stores them; loss_total[0] += beta * loss_aux[0] when loss_total is given. */
+int b200gnn_gsp_operands_f32(const int32_t* inds, int64_t S, int64_t P, int kernel, const float* pre_s, const float* bn_s,
+                             const float* pre_t, const float* bn_t, float eps, float* x_s, float* x_t, float* norm_s,
+                             float* norm_t, void* stream);
+int b200gnn_gsp_backward_f32(const int32_t* inds, int64_t S, int64_t P, int kernel, const float* g_s, const float* g_t,
+                             const float* x_s, const float* x_t, const float* norm_s, const float* norm_t, const float* rc_s,
+                             const float* rc_t, float eps, const float* pre_s, const float* bn_s, const float* pre_t,
+                             const float* bn_t, float beta, float* dz_s, float* dz_t, float* part_s, float* part_t,
+                             const float* loss_aux, float* loss_total, void* stream);
 /* y[i,:] += alpha * coef[i] * x[i,:] */
 int b200gnn_row_axpy_f32(const float* x, const float* coef, int64_t n, int64_t F,
                          float alpha, float* y, void* stream);
