@@ -22,6 +22,7 @@ import torch
 
 from . import lib, ops
 from .sparse import CsrGraph, SparseTensor
+from .trainer import FlatParams, FullBatchStudent, one_objective
 
 
 def gcn_norm(adj: SparseTensor) -> SparseTensor:
@@ -47,7 +48,7 @@ def _is_symmetric(adj: SparseTensor) -> bool:
     return bool(same)
 
 
-class GCNStudentTrainer:
+class GCNStudentTrainer(FullBatchStudent):
     """State + fused step of an L-layer GCN student on one GPU."""
 
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
@@ -59,10 +60,7 @@ class GCNStudentTrainer:
         G-CRD, one CUDA graph); lsp: an lsp.LSP run the same way (kd or supervised + beta * LSP); gsp: a gsp.GSP, the
         projection heads of G-CRD with the pairwise-similarity loss (kd or supervised + beta * GSP); at most one of the three,
         and None for all leaves the step as it is."""
-        if gcrd is not None and lsp is not None:
-            raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
-        if gsp is not None and (gcrd is not None or lsp is not None):
-            raise ValueError("gsp= and the gcrd= / lsp= objective are two auxiliary losses; pass one")
+        self.objective = one_objective(gcrd, lsp, gsp)
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         self.device = adj.device
         self.dims, self.L = list(dims), len(dims) - 1
@@ -91,38 +89,21 @@ class GCNStudentTrainer:
         self.nnz = self.G.nnz
 
         # ---- flat parameters: per layer W [in,out], b [out]; per hidden layer gamma, beta
-        sizes = []
+        shapes = []
         for l in range(self.L):
-            sizes += [dims[l] * dims[l + 1], dims[l + 1]]
+            shapes += [(dims[l], dims[l + 1]), (dims[l + 1],)]
             if l < self.L - 1:
-                sizes += [dims[l + 1], dims[l + 1]]
-        n_par = sum(sizes)
+                shapes += [(dims[l + 1],), (dims[l + 1],)]
         dev = self.device
-        self.params = torch.zeros(n_par, device=dev)
-        # gradients and the three loss scalars share one buffer (padded to 16 bytes): the multi-GPU engines exchange and
-        # reduce both with a single launch
-        self.n_par_pad = (n_par + 3) // 4 * 4
-        self._grads_buf = torch.zeros(self.n_par_pad + 4, device=dev)
-        self.grads = self._grads_buf[:n_par]
-        self.exp_avg = torch.zeros(n_par, device=dev)
-        self.exp_avg_sq = torch.zeros(n_par, device=dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.store = FlatParams(shapes, dev).attach(self)
         self.W, self.b, self.gamma, self.beta = [], [], [], []
         self.gW, self.gb, self.ggamma, self.gbeta = [], [], [], []
-        off = 0
-
-        def take(n, shape):
-            nonlocal off
-            v = (self.params[off:off + n].view(shape), self.grads[off:off + n].view(shape))
-            off += n
-            return v
+        views = iter(self.store.views)
         for l in range(self.L):
-            w, gw = take(dims[l] * dims[l + 1], (dims[l], dims[l + 1]))
-            b, gb = take(dims[l + 1], (dims[l + 1],))
+            (w, gw), (b, gb) = next(views), next(views)
             self.W.append(w); self.gW.append(gw); self.b.append(b); self.gb.append(gb)
             if l < self.L - 1:
-                g, gg = take(dims[l + 1], (dims[l + 1],))
-                be, gbe = take(dims[l + 1], (dims[l + 1],))
+                (g, gg), (be, gbe) = next(views), next(views)
                 self.gamma.append(g); self.ggamma.append(gg); self.beta.append(be); self.gbeta.append(gbe)
         # tf32 hi/lo splits of the weights for the wgmma GEMM: W^T [out,in] feeds the forward (C = X W),
         # W [in,out] feeds the input gradient (dX = dH W^T); refreshed every step (a few KB).
@@ -176,9 +157,7 @@ class GCNStudentTrainer:
         self._act_stale = False            # A[l] not yet materialised for the last forward
         self._fwd_fused = False            # the last forward left its activations to the fused kernels
         self._ev_bits = torch.cuda.Event()
-        self.loss_out = self._grads_buf[self.n_par_pad:self.n_par_pad + 3]
         self.kd_part = torch.empty(2 * int(lib.load().b200gnn_kd_partials(N)), device=dev)
-        self._graph = None
         # weight gradients only feed Adam: they run on a side stream next to the BN/ReLU backward passes and the next
         # aggregation (parallel branches of the captured graph)
         self.overlap_wgrad = overlap_wgrad
@@ -187,8 +166,6 @@ class GCNStudentTrainer:
         self._static: Dict[str, torch.Tensor] = {}
         for k in set(dims[1:]):
             self._part(k); self._coef(k)
-        # the auxiliary loss run inside the step, if any
-        self.objective = next((o for o in (gcrd, lsp, gsp) if o is not None), None)
         if self.objective is not None:
             self.objective.bind(self)
 
@@ -248,9 +225,6 @@ class GCNStudentTrainer:
     def out_feat(self) -> torch.Tensor:
         """The reference's ``model.out_feat`` (arxiv_pyg/gnn.py:51): output of the last hidden layer."""
         return self.A[-1]
-
-    def dropout_offset(self, layer: int, step: int) -> int:
-        return layer + step * self.L
 
     def forward(self, x: torch.Tensor, training: bool = True) -> torch.Tensor:
         """Returns logits [N,C]; hidden activations stay in self.A (self.A[-1] is the reference's model.out_feat)."""
@@ -411,97 +385,12 @@ class GCNStudentTrainer:
         else:
             torch.mm(inp.t(), d_out, out=self.gW[l])
 
-    def _part(self, k: int) -> torch.Tensor:
-        key = f"part{k}"
-        if key not in self._static:
-            self._static[key] = torch.empty(self.rs, 2, k, device=self.device)
-        return self._static[key]
-
-    def _coef(self, k: int) -> torch.Tensor:
-        key = f"coef{k}"
-        if key not in self._static:
-            self._static[key] = torch.empty(3, k, device=self.device)
-        return self._static[key]
-
-    def _step_impl(self, x, y, train_idx, teacher_logits, sample=None):
-        logits = self.forward(x, training=True)
-        self.dY[-1].zero_()
-        ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],
-                            loss_out=self.loss_out, partial=self.kd_part)
-        if self.objective is None:
-            self.backward(x)
-            ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-            return
-        self.backward(x, d_out_feat=self.objective.forward_backward(self, sample))
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.objective.optimizer_step(self.lr)
-
-    def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
-                   sample: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """One reference ``train()`` call: kd if teacher_logits is given, else supervised (arxiv_pyg/gnn.py:102-195), and
-        with ``aux`` the kd + beta*aux form of gnn_kd_and_aux.py:100-189 — ``aux(out_feat)`` receives the [N, H] output
-        of the last hidden layer (the reference's ``model.out_feat``, requires_grad) and returns the auxiliary loss, e.g.
-        ``lambda f: criterion.lpw_criterion(z, y, f[idx], t_feat[idx], edge_index, "cosine", 1)[2]`` or a projection head +
-        ``nce_criterion``; parameters of such heads get their gradients through torch autograd and stay with the caller's
-        optimizer.  Returns the device tensor [loss, loss_cls, loss_kd] (+ beta*aux folded into loss); no host sync.
-        With a G-CRD, LSP or GSP object (constructor) the step includes it (loss[0] += beta * loss_aux, value in its loss_aux);
-        ``sample`` (positions into train_idx, [S]) then replaces the G-CRD / GSP on-device row draw."""
-        if sample is not None and self.objective is None:
-            raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
-        if aux is None:
-            self._step_impl(x, y, train_idx, teacher_logits, *(() if sample is None else (sample,)))
-            return self.loss_out
-        if self.objective is not None:
-            raise ValueError("aux= and the trainer's G-CRD / LSP objective are two auxiliary losses; pass one")
-        logits = self.forward(x, training=True)
-        self.dY[-1].zero_()
-        ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],
-                            loss_out=self.loss_out, partial=self.kd_part)
-        feat = self.out_feat().detach().requires_grad_(True)
-        with torch.enable_grad():
-            loss_aux = aux(feat)
-            (loss_aux * beta).backward()
-        d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
-        self.backward(x, d_out_feat=d_feat.contiguous())
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.loss_aux = loss_aux.detach()
-        self.loss_out[0].add_(self.loss_aux * beta)
-        return self.loss_out
-
-    # ------------------------------------------------------------------ CUDA graph
-    def capture(self, x, y, train_idx, teacher_logits=None, warmup: int = 2, key: int = 0):
-        """Capture the step on static input buffers; afterwards ``replay(key)`` runs one full step.
-        Several input-buffer sets can be captured (key = 0, 1, ...) so that uploads of the next step's inputs overlap
-        the current step (activations and parameters are shared between the graphs)."""
-        self._static.update(x=x, y=y, train_idx=train_idx, teacher=teacher_logits)
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                self._step_impl(x, y, train_idx, teacher_logits)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        if self._graph is None:
-            self._graph = {}
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._step_impl(x, y, train_idx, teacher_logits)
-        self._graph[key] = g
-        return self
-
     def replay(self, key: int = 0) -> torch.Tensor:
-        self._graph[key].replay()
+        super().replay(key)
         self._act_stale = self.fuse_act
         return self.loss_out
 
     # ------------------------------------------------------------------ accounting
-    def launches_per_step(self) -> int:
-        """b200gnn kernel launches in one training step (counted, not estimated)."""
-        before = lib.launch_count()
-        st = self._static
-        self._step_impl(st["x"], st["y"], st["train_idx"], st["teacher"])
-        return lib.launch_count() - before
-
     def aggregations_per_step(self) -> Dict[int, int]:
         """width -> number of SpMM launches of that width in one training step."""
         out: Dict[int, int] = {}

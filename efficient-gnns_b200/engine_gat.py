@@ -31,6 +31,7 @@ import torch
 from . import lib, ops
 from .nn import _csr2csc_i32, _hub_args
 from .sparse import SparseTensor
+from .trainer import FlatParams, FullBatchStudent
 
 WGRAD_BLOCK = 512          # widest output block of one weight-gradient launch
 
@@ -43,7 +44,7 @@ def padded_head(H: int, D: int, hidden: bool = True) -> int:
     return Dp
 
 
-class GATTrainer:
+class GATTrainer(FullBatchStudent):
     """State + fused step of the reference's GAT on one GPU (adj rows = destinations, bidirected with self-loops)."""
 
     def __init__(self, adj: SparseTensor, in_feats: int, n_classes: int, n_hidden: int, n_layers: int, n_heads: int,
@@ -98,45 +99,28 @@ class GATTrainer:
 
         # ---- flat parameters: per layer the column blocks of W_fc and W_res ([in, block], so that a weight gradient is one
         # contiguous output), attn_l, attn_r, BatchNorm gamma / beta; bias_last at the end
-        sizes = []
+        shapes = []
         for l in range(L):
-            sizes += [self.Kin[l] * nb for _ in range(2) for _, nb in self.blocks[l]] + [self.K[l]] * (2 if self.use_attn_dst else 1)
-            if l < L - 1:
-                sizes += [self.K[l]] * 2
-        sizes.append(self.K[-1])
-        n_par = sum(sizes)
-        self.params = torch.zeros(n_par, device=dev)
-        self.n_par_pad = (n_par + 3) // 4 * 4
-        self._grads_buf = torch.zeros(self.n_par_pad + 4, device=dev)
-        self.grads = self._grads_buf[:n_par]
-        self.exp_avg, self.exp_avg_sq = torch.zeros(n_par, device=dev), torch.zeros(n_par, device=dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)
-        off = 0
-
-        def take(n, shape):
-            nonlocal off
-            v = (self.params[off:off + n].view(shape), self.grads[off:off + n].view(shape))
-            off += n
-            return v
+            shapes += [(self.Kin[l], nb) for _ in range(2) for _, nb in self.blocks[l]]
+            shapes += [(self.K[l],)] * ((2 if self.use_attn_dst else 1) + (2 if l < L - 1 else 0))
+        shapes.append((self.K[-1],))
+        self.store = FlatParams(shapes, dev).attach(self)
+        views = iter(self.store.views)
         self.Wfc, self.Wres, self.gWfc, self.gWres = [], [], [], []
         self.attn_l, self.attn_r, self.g_attn_l, self.g_attn_r = [], [], [], []
         self.gamma, self.beta, self.ggamma, self.gbeta = [], [], [], []
         for l in range(L):
             for W, gW in ((self.Wfc, self.gWfc), (self.Wres, self.gWres)):
-                pairs = [take(self.Kin[l] * nb, (self.Kin[l], nb)) for _, nb in self.blocks[l]]
+                pairs = [next(views) for _ in self.blocks[l]]
                 W.append([p for p, _ in pairs]); gW.append([g for _, g in pairs])
-            a, ga = take(self.K[l], (self.K[l],))
+            a, ga = next(views)
             self.attn_l.append(a); self.g_attn_l.append(ga)
-            if self.use_attn_dst:
-                a, ga = take(self.K[l], (self.K[l],))
-                self.attn_r.append(a); self.g_attn_r.append(ga)
-            else:
-                self.attn_r.append(None); self.g_attn_r.append(None)
+            a, ga = next(views) if self.use_attn_dst else (None, None)
+            self.attn_r.append(a); self.g_attn_r.append(ga)
             if l < L - 1:
-                g, gg = take(self.K[l], (self.K[l],))
-                b, gb = take(self.K[l], (self.K[l],))
+                (g, gg), (b, gb) = next(views), next(views)
                 self.gamma.append(g); self.ggamma.append(gg); self.beta.append(b); self.gbeta.append(gb)
-        self.bias_last, self.g_bias_last = take(self.K[-1], (self.K[-1],))
+        self.bias_last, self.g_bias_last = next(views)
         # tf32 hi / lo splits, refreshed every step: [W_fc | W_res]^T stacked [2K, in] feeds the forward GEMM, the blocks as
         # stored ([in, block]) feed the input-gradient GEMMs
         self.Wt_split = [tuple(torch.empty(2 * self.K[l], self.Kin[l], device=dev) for _ in range(2)) for l in range(L)]
@@ -178,11 +162,9 @@ class GATTrainer:
         self.in_bits = torch.full((1, N, (self.in_feats + 31) // 32), -1, dtype=torch.int32, device=dev)
         self.one = torch.ones(1, device=dev)                                       # PReLU slope 1: "dropout only"
         self.edge_keep = [torch.ones((self.nnz + 3) // 4 * 4, dtype=torch.uint8, device=dev) for _ in range(L)]
-        self.loss_out = self._grads_buf[self.n_par_pad:self.n_par_pad + 3]
         self.kd_part = torch.empty(2 * int(lib.load().b200gnn_kd_partials(N)), device=dev)
         self._side = torch.cuda.Stream(device=dev)
         self._ev_fork, self._ev_join, self._ev_bits = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
-        self._graph: Dict[int, torch.cuda.CUDAGraph] = {}
         self._static: Dict[str, torch.Tensor] = {}
         self._training = False
 
@@ -407,7 +389,8 @@ class GATTrainer:
             lib.check(rc, "gemm_tf32x3 (input gradient)")
 
     def backward(self, x: torch.Tensor, d_out_feat: Optional[torch.Tensor] = None):
-        """Consumes self.dY[-1] (d loss / d logits, stored layout) and optionally d loss / d out_feat; fills self.grads."""
+        """Consumes self.dY[-1] (d loss / d logits, stored layout) and optionally d loss / d out_feat (out_feat()'s layout);
+        fills self.grads."""
         L_ = lib.load()
         N = self.N
         ops.col_sum(self.dY[-1], out=self.g_bias_last, partial=self.row_part)
@@ -428,7 +411,10 @@ class GATTrainer:
                                self.g_attn_l[l], self.g_attn_r[l], partial=self.score_part)
             if l > 0:
                 seeded = d_out_feat is not None and l == self.L - 1
-                if seeded:
+                if seeded and self.Dp[0] != self.Dl[0]:             # into the stored columns, padding zero
+                    self.dY[l - 1].zero_()
+                    self.dY[l - 1][:, self._cols(self.L - 2)] = d_out_feat
+                elif seeded:
                     self.dY[l - 1].copy_(d_out_feat)
                 self._dgrad(l, seeded)
             self._ev_fork.record(torch.cuda.current_stream())     # weight gradients only feed Adam: side stream
@@ -450,8 +436,10 @@ class GATTrainer:
         torch.cuda.current_stream().wait_event(self._ev_join)
 
     # ------------------------------------------------------------------ step
-    def _loss(self, logits, y, train_idx, teacher_logits):
-        """Fused CE / logit-KD over rows train_idx; d loss / d logits into the stored-layout dY[-1] (padding stays zero)."""
+    def _loss(self, x, y, train_idx, teacher_logits):
+        """Training forward, then the fused CE / logit-KD over rows train_idx; d loss / d logits into the stored-layout dY[-1]
+        (padding stays zero)."""
+        logits = self.forward(x, training=True)
         self.dY[-1].zero_()
         t = teacher_logits
         lib.check(lib.load().b200gnn_kd_loss_fwd_bwd_f32(
@@ -460,66 +448,12 @@ class GATTrainer:
             0 if t is None else t.stride(0), self.n_classes, self.alpha, self.kd_T, 0, self.dY[-1].data_ptr(), self.dY[-1].stride(0),
             self.loss_out.data_ptr(), self.kd_part.data_ptr(), lib.stream_ptr()), "kd_loss_fwd_bwd_f32")
 
-    def _step_impl(self, x, y, train_idx, teacher_logits):
-        logits = self.forward(x, training=True)
-        self._loss(logits, y, train_idx, teacher_logits)
-        self.backward(x)
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-
-    def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0) -> torch.Tensor:
-        """One training step: cross-entropy, or the kd_criterion mix when teacher logits are given; ``aux(out_feat)`` adds
-        beta * aux and its gradient seeds the backward at the last hidden activation (the interface of
-        GCNStudentTrainer.train_step).  Returns the device tensor [loss, loss_cls, loss_kd]; no host sync."""
-        if aux is None:
-            self._step_impl(x, y, train_idx, teacher_logits)
-            return self.loss_out
-        logits = self.forward(x, training=True)
-        self._loss(logits, y, train_idx, teacher_logits)
-        feat = self.out_feat().detach().requires_grad_(True)
-        with torch.enable_grad():
-            loss_aux = aux(feat)
-            (loss_aux * beta).backward()
-        d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
-        if self.Dp[0] != self.Dl[0]:
-            full = torch.zeros(self.N, self.K[0], device=self.device)
-            full[:, self._cols(self.L - 2)] = d_feat
-            d_feat = full
-        self.backward(x, d_out_feat=d_feat.contiguous())
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.loss_aux = loss_aux.detach()
-        self.loss_out[0].add_(self.loss_aux * beta)
-        return self.loss_out
-
-    # ------------------------------------------------------------------ CUDA graph
-    def capture(self, x, y, train_idx, teacher_logits=None, warmup: int = 2, key: int = 0):
-        """Capture the supervised / KD step on static input buffers; ``replay(key)`` then runs one full step."""
-        self._static.update(x=x, y=y, train_idx=train_idx, teacher=teacher_logits)
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                self._step_impl(x, y, train_idx, teacher_logits)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._step_impl(x, y, train_idx, teacher_logits)
-        self._graph[key] = g
-        return self
-
     def replay(self, key: int = 0) -> torch.Tensor:
-        self._graph[key].replay()
+        super().replay(key)
         self._training = True
         return self.loss_out
 
     # ------------------------------------------------------------------ accounting
-    def launches_per_step(self) -> int:
-        """b200gnn kernel launches in one training step (counted, not estimated); advances the state by one step."""
-        before = lib.launch_count()
-        st = self._static
-        self._step_impl(st["x"], st["y"], st["train_idx"], st["teacher"])
-        return lib.launch_count() - before
-
     def algorithmic_bytes(self) -> Dict[str, int]:
         """Compulsory HBM bytes per launch of the sparse kernels of one layer at the hidden width, from shapes:
         aggregation = read ft + write Y + read res + coefficients and indices; scores = one read of ft + el, er."""

@@ -28,6 +28,7 @@ import torch
 from . import ops
 from .engine_gat import GATTrainer
 from .sparse import SparseTensor
+from .trainer import capture_graph
 
 HISTORY_COLUMNS = ("acc", "train_acc", "val_acc", "test_acc", "loss", "train_loss", "val_loss", "test_loss")
 WARMUP_EPOCHS = 50          # adjust_learning_rate, gat.py:110-113
@@ -142,11 +143,7 @@ class GATTeacherTrainer(GATTrainer):
 
     def capture(self):
         """Record one epoch (train, evaluate, snapshot, history row) as one CUDA graph.  Capturing runs nothing."""
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._epoch_impl()
-        self._epoch_graph = g
+        self._epoch_graph = capture_graph(self._epoch_impl, warmup=0)
         return self
 
     def replay(self) -> torch.Tensor:
@@ -171,13 +168,6 @@ class GATTeacherTrainer(GATTrainer):
         return hist.cpu()
 
     # ------------------------------------------------------------------ reference-format state
-    def _like(self, buf: torch.Tensor, t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-        """The view of a flat buffer laid out like self.params at the place of parameter view t."""
-        if t is None:
-            return None
-        off = (t.data_ptr() - self.params.data_ptr()) // t.element_size()
-        return buf[off:off + t.numel()].view(t.shape)
-
     def _reference_order(self, sd: Dict[str, torch.Tensor], buffers: bool) -> "OrderedDict[str, torch.Tensor]":
         """Keys in the order of the reference module's state_dict() (parameters() when buffers is False): per GATConv its own
         attn_l, attn_r, then fc.weight, res_fc.weight; per BatchNorm weight, bias (, running statistics, batch count)."""
@@ -202,11 +192,11 @@ class GATTeacherTrainer(GATTrainer):
 
     def named_square_avg(self) -> "OrderedDict[str, torch.Tensor]":
         """RMSprop's square_avg under the parameter names, in parameters() order."""
-        b, lk = self.square_avg, self._like
-        return self._reference_order(self._export([[lk(b, t) for t in W] for W in self.Wfc], [[lk(b, t) for t in W] for W in self.Wres],
-                                                  [lk(b, t) for t in self.attn_l], [lk(b, t) for t in self.attn_r],
-                                                  [lk(b, t) for t in self.gamma], [lk(b, t) for t in self.beta],
-                                                  lk(b, self.bias_last)), buffers=False)
+        lk = lambda t: None if t is None else self.store.like(self.square_avg, t)          # noqa: E731
+        return self._reference_order(self._export([[lk(t) for t in W] for W in self.Wfc], [[lk(t) for t in W] for W in self.Wres],
+                                                  [lk(t) for t in self.attn_l], [lk(t) for t in self.attn_r],
+                                                  [lk(t) for t in self.gamma], [lk(t) for t in self.beta], lk(self.bias_last)),
+                                     buffers=False)
 
     def model_state_dict(self) -> "OrderedDict[str, torch.Tensor]":
         """The reference module's state_dict() on the CPU, num_batches_tracked included (one per training forward)."""

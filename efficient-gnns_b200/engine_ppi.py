@@ -29,6 +29,7 @@ import torch
 
 from . import lib, ops
 from .nn import _as_adj, _csr2csc_i32, _fill_diag_pattern, _hub_args
+from .trainer import FlatParams, aux_grad, capture_graph
 
 WGRAD_BLOCK = 512          # widest output block of one weight-gradient launch
 STUDENT_LAYERS = [(2, 68, True)] * 4 + [(2, 121, False)]     # ppi_pyg/gnn.py:50-83
@@ -129,35 +130,25 @@ class PPIGATTrainer:
 
         # ---- flat parameters, per layer: the column blocks of [W_lin | W_skip] as [in, block] (a weight gradient is one
         # contiguous output), att_l, att_r, a zero vector and b_lin (together the GEMM's bias [0 | b_lin]), b_conv
-        sizes = []
+        shapes = []
         for l in range(L):
-            sizes += [self.Kin[l] * nb for _, nb in self.blocks[l]] + [self.Kft[l]] * 3 + [self.Kout[l]] * 2
-        n_par = sum(sizes)
-        self.params = torch.zeros(n_par, device=dev)
-        self.grads = torch.zeros(n_par, device=dev)
-        self.exp_avg, self.exp_avg_sq = torch.zeros(n_par, device=dev), torch.zeros(n_par, device=dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)
-        off = 0
-
-        def take(n, shape):
-            nonlocal off
-            v = (self.params[off:off + n].view(shape), self.grads[off:off + n].view(shape))
-            off += n
-            return v
+            shapes += [(self.Kin[l], nb) for _, nb in self.blocks[l]] + [(self.Kft[l],)] * 3 + [(self.Kout[l],)] * 2
+        self.store = FlatParams(shapes, dev).attach(self)
+        views = iter(self.store.views)
         self.W, self.gW, self.att_l, self.g_att_l, self.att_r, self.g_att_r = [], [], [], [], [], []
         self.gemm_bias, self.b_lin, self.g_b_lin, self.b_conv, self.g_b_conv = [], [], [], [], []
         for l in range(L):
-            pairs = [take(self.Kin[l] * nb, (self.Kin[l], nb)) for _, nb in self.blocks[l]]
+            pairs = [next(views) for _ in self.blocks[l]]
             self.W.append([p for p, _ in pairs]); self.gW.append([g for _, g in pairs])
             for P, G_ in ((self.att_l, self.g_att_l), (self.att_r, self.g_att_r)):
-                p, g = take(self.Kft[l], (self.Kft[l],))
+                p, g = next(views)
                 P.append(p); G_.append(g)
-            o0 = off
-            take(self.Kft[l], (self.Kft[l],))
-            p, g = take(self.Kout[l], (self.Kout[l],))
+            zero, _ = next(views)
+            p, g = next(views)
             self.b_lin.append(p); self.g_b_lin.append(g)
-            self.gemm_bias.append(self.params[o0:off])
-            p, g = take(self.Kout[l], (self.Kout[l],))
+            o0 = self.store.offset(zero)
+            self.gemm_bias.append(self.params[o0:o0 + self.Kft[l] + self.Kout[l]])
+            p, g = next(views)
             self.b_conv.append(p); self.g_b_conv.append(g)
         # tf32 hi / lo splits, refreshed every step: [W_lin | W_skip]^T [Ktot, in] feeds the forward GEMM, [in, Ktot] the
         # input-gradient GEMM
@@ -183,7 +174,6 @@ class PPIGATTrainer:
         self.score_part = torch.empty(ops.gat_scores_slots(n_max), 2, max(self.Kft), device=dev)
         self.col_part = torch.empty(int(lib.load().b200gnn_col_sum_ld_slots(n_max)) * max(self.Kout), device=dev)
         self.tail_part = torch.empty(2 * int(lib.load().b200gnn_ppi_tail_slots(n_max)), dtype=torch.float64, device=dev)
-        self.loss_out = torch.zeros(3, device=dev)
         self._side = torch.cuda.Stream(device=dev)
         self._ev_fork, self._ev_join = torch.cuda.Event(), torch.cuda.Event()
         self._graph: Dict[int, torch.cuda.CUDAGraph] = {}
@@ -357,37 +347,28 @@ class PPIGATTrainer:
     def _teacher(self, i: int) -> Optional[torch.Tensor]:
         return None if self.teacher_logits is None else self.teacher_logits[i]
 
-    def _step_impl(self, i: int):
+    def _step_impl(self, i: int, aux=None, beta: float = 1.0):
         g = self.graphs[i]
         b = self.bufs.view(g.n, g.nnz)
         self._forward(g, b, self.x[i], self.y[i], self._teacher(i))
-        self._backward(g, b, self.x[i])
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
         self._last = (g, b)
+        d_feat = None
+        if aux is not None:
+            d, loss_aux = aux_grad(self.out_feat(), aux, beta)
+            d_feat = torch.zeros(g.n, self.Kout[-2], device=self.device)        # into the stored columns, padding zero
+            d_feat[:, self._cols(self.L - 2)] = d
+        self._backward(g, b, self.x[i], d_out_feat=d_feat)
+        self.store.adam(self.lr)
+        if aux is not None:
+            self.loss_out[0].add_(loss_aux * beta)
+            self.loss_out[2].copy_(loss_aux)
 
     def train_step(self, i: int, aux=None, beta: float = 1.0) -> torch.Tensor:
         """One step on training graph i: BCE, or kd_criterion when teacher logits were given.  ``aux(out_feat)`` (the [n, hidden]
         activation of layer L-2, requires_grad) returns an auxiliary loss that enters as loss + beta * aux and seeds the backward
         at out_feat (gnn.py:213-265); the teacher's out_feat for graph i is ``self.teacher_feat[i]``.  Returns the device tensor
         [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's value when given); no host sync."""
-        if aux is None:
-            self._step_impl(i)
-            return self.loss_out
-        g = self.graphs[i]
-        b = self.bufs.view(g.n, g.nnz)
-        self._forward(g, b, self.x[i], self.y[i], self._teacher(i))
-        self._last = (g, b)
-        feat = self.out_feat().detach().requires_grad_(True)
-        with torch.enable_grad():
-            loss_aux = aux(feat)
-            (loss_aux * beta).backward()
-        d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
-        full = torch.zeros(g.n, self.Kout[-2], device=self.device)
-        full[:, self._cols(self.L - 2)] = d_feat
-        self._backward(g, b, self.x[i], d_out_feat=full)
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.loss_out[0].add_(loss_aux.detach() * beta)
-        self.loss_out[2].copy_(loss_aux.detach())
+        self._step_impl(i, aux, beta)
         return self.loss_out
 
     def logits(self) -> torch.Tensor:
@@ -403,22 +384,9 @@ class PPIGATTrainer:
     def capture(self, warmup: int = 1):
         """Record one CUDA graph per training graph.  Warm-up steps run on a saved copy of the parameters and Adam state,
         which is restored afterwards: capturing does not train."""
-        saved = [t.clone() for t in (self.params, self.exp_avg, self.exp_avg_sq, self.step_count)]
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                for i in range(len(self.graphs)):
-                    self._step_impl(i)
-        torch.cuda.current_stream().wait_stream(s)
-        for t, v in zip((self.params, self.exp_avg, self.exp_avg_sq, self.step_count), saved):
-            t.copy_(v)
-        torch.cuda.synchronize()
-        for i in range(len(self.graphs)):
-            cg = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(cg):
-                self._step_impl(i)
-            self._graph[i] = cg
+        with self.store.preserved():
+            for i in range(len(self.graphs)):
+                self._graph[i] = capture_graph(lambda: self._step_impl(i), warmup)
         return self
 
     def replay(self, i: int) -> torch.Tensor:

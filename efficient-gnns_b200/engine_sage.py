@@ -26,18 +26,16 @@ import torch
 
 from . import lib, ops
 from .sparse import CsrGraph, SparseTensor
+from .trainer import FlatParams, FullBatchStudent, one_objective
 
 
-class SAGEStudentTrainer:
+class SAGEStudentTrainer(FullBatchStudent):
     def __init__(self, adj: SparseTensor, dims: List[int], dropout: float = 0.5, lr: float = 0.01, seed: int = 0,
                  alpha: float = 0.9, kd_T: float = 4.0, bn_eps: float = 1e-5, bn_momentum: float = 0.1,
                  fuse_row_passes: bool = True, gcrd=None, lsp=None, gsp=None):
         """gcrd / lsp / gsp: a gcrd.GCRD, an lsp.LSP or a gsp.GSP run inside the step as engine.GCNStudentTrainer runs it;
         at most one, and None for all leaves the step as it is."""
-        if gcrd is not None and lsp is not None:
-            raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
-        if gsp is not None and (gcrd is not None or lsp is not None):
-            raise ValueError("gsp= and the gcrd= / lsp= objective are two auxiliary losses; pass one")
+        self.objective = one_objective(gcrd, lsp, gsp)
         assert adj.is_cuda(), "the engine runs on a CUDA device"
         for d in dims:
             assert d % 4 == 0 and d <= 1024, "layer widths must be multiples of 4 (128-bit rows)"
@@ -50,35 +48,21 @@ class SAGEStudentTrainer:
         self.G: CsrGraph = st.engine_csr_unweighted()         # mean over in-neighbours
         self.Gt: CsrGraph = st.engine_csc("mean")             # transpose with 1/deg(dst) weights: the mean's backward
         self.nnz = self.G.nnz
-        sizes = []
+        shapes = []
         for l in range(self.L):
-            sizes += [dims[l + 1] * dims[l], dims[l + 1], dims[l + 1] * dims[l]]      # W_l [out,in], b_l, W_r [out,in]
+            shapes += [(dims[l + 1], dims[l]), (dims[l + 1],), (dims[l + 1], dims[l])]      # W_l [out,in], b_l, W_r [out,in]
             if l < self.L - 1:
-                sizes += [dims[l + 1], dims[l + 1]]
-        n_par = sum(sizes)
-        self.params = torch.zeros(n_par, device=dev)
-        self.n_par_pad = (n_par + 3) // 4 * 4
-        self._grads_buf = torch.zeros(self.n_par_pad + 4, device=dev)
-        self.grads = self._grads_buf[:n_par]
-        self.loss_out = self._grads_buf[self.n_par_pad:self.n_par_pad + 3]
-        self.exp_avg, self.exp_avg_sq = torch.zeros(n_par, device=dev), torch.zeros(n_par, device=dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)
+                shapes += [(dims[l + 1],), (dims[l + 1],)]
+        self.store = FlatParams(shapes, dev).attach(self)
         self.Wl, self.bl, self.Wr, self.gamma, self.beta = [], [], [], [], []
         self.gWl, self.gbl, self.gWr, self.ggamma, self.gbeta = [], [], [], [], []
-        off = 0
-
-        def take(n, shape):
-            nonlocal off
-            v = (self.params[off:off + n].view(shape), self.grads[off:off + n].view(shape))
-            off += n
-            return v
+        views = iter(self.store.views)
         for l in range(self.L):
-            a, b = take(dims[l + 1] * dims[l], (dims[l + 1], dims[l])); self.Wl.append(a); self.gWl.append(b)
-            a, b = take(dims[l + 1], (dims[l + 1],)); self.bl.append(a); self.gbl.append(b)
-            a, b = take(dims[l + 1] * dims[l], (dims[l + 1], dims[l])); self.Wr.append(a); self.gWr.append(b)
+            for P, G_ in ((self.Wl, self.gWl), (self.bl, self.gbl), (self.Wr, self.gWr)):
+                a, b = next(views); P.append(a); G_.append(b)
             if l < self.L - 1:
-                a, b = take(dims[l + 1], (dims[l + 1],)); self.gamma.append(a); self.ggamma.append(b)
-                a, b = take(dims[l + 1], (dims[l + 1],)); self.beta.append(a); self.gbeta.append(b)
+                for P, G_ in ((self.gamma, self.ggamma), (self.beta, self.gbeta)):
+                    a, b = next(views); P.append(a); G_.append(b)
         self.running_mean = [torch.zeros(d, device=dev) for d in dims[1:-1]]
         self.running_var = [torch.ones(d, device=dev) for d in dims[1:-1]]
         buf = lambda k: torch.zeros(N, k, device=dev)
@@ -99,10 +83,7 @@ class SAGEStudentTrainer:
         wg = [(dims[l], dims[l + 1]) for l in range(self.L) if ops.wgrad_supported(dims[l], dims[l + 1])]
         self.wgrad_ws = torch.empty(max(ops.wgrad_workspace_floats(a, b) for a, b in wg), device=dev) if wg else None
         self.loss_aux = None
-        self._graph = None
         self.reset_parameters(seed)
-        # the auxiliary loss run inside the step, if any
-        self.objective = next((o for o in (gcrd, lsp, gsp) if o is not None), None)
         if self.objective is not None:
             self.objective.bind(self)
 
@@ -141,18 +122,6 @@ class SAGEStudentTrainer:
             self.gamma[l].copy_(sd[f"bns.{l}.weight"]); self.beta[l].copy_(sd[f"bns.{l}.bias"])
 
     # ------------------------------------------------------------------ helpers
-    def _part(self, k):
-        key = f"part{k}"
-        if key not in self._static:
-            self._static[key] = torch.empty(self.rs, 2, k, device=self.device)
-        return self._static[key]
-
-    def _coef(self, k):
-        key = f"coef{k}"
-        if key not in self._static:
-            self._static[key] = torch.empty(3, k, device=self.device)
-        return self._static[key]
-
     def _split(self, w: torch.Tensor, transpose: bool, key: str):
         shape = (w.shape[1], w.shape[0]) if transpose else tuple(w.shape)
         if key not in self.split:
@@ -175,9 +144,6 @@ class SAGEStudentTrainer:
 
     def out_feat(self) -> torch.Tensor:
         return self.A[-1]
-
-    def dropout_offset(self, layer: int, step: int) -> int:
-        return layer + step * self.L
 
     # ------------------------------------------------------------------ forward / backward
     def forward(self, x: torch.Tensor, training: bool = True) -> torch.Tensor:
@@ -240,61 +206,3 @@ class SAGEStudentTrainer:
             ops.bn_act_bwd(d_prev, self.A[l - 1], self.Y[l - 1], self.bn[l - 1][0], self.bn[l - 1][1], self.gamma[l - 1], self.p,
                            d_y=self.dY[l - 1], d_gamma=self.ggamma[l - 1], d_beta=self.gbeta[l - 1], partial=self._part(kp),
                            coef=self._coef(kp), want_dbias=False)
-
-    def _loss(self, x, y, train_idx, teacher_logits):
-        logits = self.forward(x, training=True)
-        self.dY[-1].zero_()
-        ops.kd_loss_fwd_bwd(logits, y, train_idx, teacher_logits, self.alpha, self.kd_T, d_logits=self.dY[-1],
-                            loss_out=self.loss_out, partial=self.kd_part)
-
-    def _step_impl(self, x, y, train_idx, teacher_logits, sample=None):
-        self._loss(x, y, train_idx, teacher_logits)
-        if self.objective is None:
-            self.backward(x)
-            ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-            return
-        self.backward(x, d_out_feat=self.objective.forward_backward(self, sample))
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.objective.optimizer_step(self.lr)
-
-    def train_step(self, x, y, train_idx, teacher_logits=None, aux=None, beta: float = 1.0,
-                   sample: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """One reference ``train()`` call for ``--gnn sage``: supervised / kd, or kd + beta*aux with ``aux(out_feat)`` as in
-        engine.GCNStudentTrainer.train_step, or with the G-CRD, LSP or GSP object of the constructor (``sample`` as there).
-        Returns the device tensor [loss, loss_cls, loss_kd]."""
-        if sample is not None and self.objective is None:
-            raise ValueError("sample= is the G-CRD row sample; this trainer has no G-CRD head")
-        if aux is None:
-            self._step_impl(x, y, train_idx, teacher_logits, *(() if sample is None else (sample,)))
-            return self.loss_out
-        if self.objective is not None:
-            raise ValueError("aux= and the trainer's G-CRD / LSP objective are two auxiliary losses; pass one")
-        self._loss(x, y, train_idx, teacher_logits)
-        feat = self.out_feat().detach().requires_grad_(True)
-        with torch.enable_grad():
-            loss_aux = aux(feat)
-            (loss_aux * beta).backward()
-        d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
-        self.backward(x, d_out_feat=d_feat)
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.loss_aux = loss_aux.detach()
-        self.loss_out[0].add_(self.loss_aux * beta)
-        return self.loss_out
-
-    # ------------------------------------------------------------------ CUDA graph
-    def capture(self, x, y, train_idx, teacher_logits=None, warmup: int = 2):
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                self._step_impl(x, y, train_idx, teacher_logits)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        self._graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self._graph):
-            self._step_impl(x, y, train_idx, teacher_logits)
-        return self
-
-    def replay(self) -> torch.Tensor:
-        self._graph.replay()
-        return self.loss_out

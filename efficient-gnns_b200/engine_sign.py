@@ -24,6 +24,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import lib, ops
+from .trainer import FlatParams, aux_grad, capture_graph
 
 
 class _Acts:
@@ -119,25 +120,15 @@ class SIGNStudentTrainer:
             shapes.append(("h_slope", (H,)))
             shapes.append(("p_slope", (1,)))
         shapes.append(("slope", (1,)))
-        n_par = sum(math.prod(s) for _, s in shapes)
-        self.params = torch.zeros(n_par, device=dev)
-        self._grads_buf = torch.zeros(n_par + 4, device=dev)
-        self.grads = self._grads_buf[:n_par]
-        self.loss_out = self._grads_buf[n_par:n_par + 3]
-        self.exp_avg = torch.zeros(n_par, device=dev)
-        self.exp_avg_sq = torch.zeros(n_par, device=dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.store = FlatParams([s for _, s in shapes], dev).attach(self)
         self.P: Dict[str, torch.Tensor] = {}
         self.G: Dict[str, torch.Tensor] = {}
-        off = 0
-        for name, s in shapes:
-            k = math.prod(s)
-            self.P[name], self.G[name] = self.params[off:off + k].view(s), self.grads[off:off + k].view(s)
-            off += k
+        for (name, _), (p, g) in zip(shapes, self.store.views):
+            self.P[name], self.G[name] = p, g
         # tf32 (hi, lo) splits: the input-gradient GEMMs read every weight in its stored layout (one launch over the flat
         # buffer); the forward GEMMs read Wᵀ, split per layer
-        self._split_hi = torch.empty(n_par, device=dev)
-        self._split_lo = torch.empty(n_par, device=dev)
+        self._split_hi = torch.empty_like(self.params)
+        self._split_lo = torch.empty_like(self.params)
         self._fsplit = {name: (torch.empty(s[1], s[0], device=dev), torch.empty(s[1], s[0], device=dev))
                         for name, s in shapes if ".W" in name}
         wg = [(F, hid), (hid, hid), (hid, C), (H * hid if H * hid <= 2048 else ops.WGRAD_PRELU_BLOCK, hid if ff > 1 else C)]
@@ -235,11 +226,7 @@ class SIGNStudentTrainer:
 
     def _bw(self, key: str):
         """(hi, lo) of the stored [in, out] weight: the B operand of the input-gradient GEMM."""
-        w = self.P[key]
-        off = w.data_ptr() - self.params.data_ptr()
-        k = w.numel()
-        s = off // 4
-        return self._split_hi[s:s + k].view(w.shape), self._split_lo[s:s + k].view(w.shape)
+        return self.store.like(self._split_hi, self.P[key]), self.store.like(self._split_lo, self.P[key])
 
     def _forward(self, a: _Acts, idx: torch.Tensor, training: bool, y=None, teacher=None) -> torch.Tensor:
         B, H, hid, ff = idx.numel(), self.H, self.hidden, self.ff
@@ -319,15 +306,20 @@ class SIGNStudentTrainer:
         if not 0 < idx.numel() <= self.batch_size:
             raise ValueError(f"batch of {idx.numel()} rows: expected 1..{self.batch_size}")
 
-    def _step_impl(self, idx, y, teacher_logits):
+    def _step_impl(self, idx, y, teacher_logits, aux=None, beta: float = 1.0):
         B = idx.numel()
         a = self._tr
         logits = self._forward(a, idx, True, y, teacher_logits)
         ops.kd_loss_fwd_bwd(logits, a.labels[:B], None, a.teacher[:B] if teacher_logits is not None else None, self.alpha,
                             self.kd_T, d_logits=a.dlogits[:B], loss_out=self.loss_out, partial=self.kd_part)
-        self._backward(B, None)
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
         self._B, self._feat_stale = B, True
+        d_feat = None
+        if aux is not None:
+            d_feat, self.loss_aux = aux_grad(self.out_feat(), aux, beta)
+        self._backward(B, d_feat)
+        self.store.adam(self.lr)
+        if aux is not None:
+            self.loss_out[0].add_(self.loss_aux * beta)
 
     def train_step(self, batch_idx: torch.Tensor, y: torch.Tensor, teacher_logits: Optional[torch.Tensor] = None, aux=None,
                    beta: float = 1.0) -> torch.Tensor:
@@ -337,24 +329,7 @@ class SIGNStudentTrainer:
         kd + beta*aux; heads inside it keep their gradients in the caller's autograd.  Returns the device tensor
         [loss, loss_cls, loss_kd] (beta*aux folded into loss); no host sync."""
         self._check_batch(batch_idx)
-        if aux is None:
-            self._step_impl(batch_idx, y, teacher_logits)
-            return self.loss_out
-        B = batch_idx.numel()
-        a = self._tr
-        logits = self._forward(a, batch_idx, True, y, teacher_logits)
-        ops.kd_loss_fwd_bwd(logits, a.labels[:B], None, a.teacher[:B] if teacher_logits is not None else None, self.alpha,
-                            self.kd_T, d_logits=a.dlogits[:B], loss_out=self.loss_out, partial=self.kd_part)
-        self._B, self._feat_stale = B, True
-        feat = self.out_feat().detach().requires_grad_(True)
-        with torch.enable_grad():
-            loss_aux = aux(feat)
-            (loss_aux * beta).backward()
-        d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
-        self._backward(B, d_feat)
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
-        self.loss_aux = loss_aux.detach()
-        self.loss_out[0].add_(self.loss_aux * beta)
+        self._step_impl(batch_idx, y, teacher_logits, aux, beta)
         return self.loss_out
 
     def out_feat(self) -> torch.Tensor:
@@ -397,21 +372,10 @@ class SIGNStudentTrainer:
     def capture(self, batch_sizes, y: torch.Tensor, teacher_logits: Optional[torch.Tensor] = None):
         """Capture one CUDA graph of the step per batch size (the batch indices are read from a static buffer).  The
         warm-up steps run on a copy of the optimiser state, which is restored: capturing does not train."""
-        saved = [t.clone() for t in (self.params, self.exp_avg, self.exp_avg_sq, self.step_count)]
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream())
-        for B in sorted(set(int(b) for b in batch_sizes)):
-            idx = self._idx_static[:B]
-            with torch.cuda.stream(s):
-                self._step_impl(idx, y, teacher_logits)
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._step_impl(idx, y, teacher_logits)
-            self._graphs[B] = g
-        for t, v in zip((self.params, self.exp_avg, self.exp_avg_sq, self.step_count), saved):
-            t.copy_(v)
+        with self.store.preserved():
+            for B in sorted(set(int(b) for b in batch_sizes)):
+                idx = self._idx_static[:B]
+                self._graphs[B] = capture_graph(lambda: self._step_impl(idx, y, teacher_logits), warmup=1)
         self._graph_inputs = (y, teacher_logits)
         self._feat_stale = False
         return self

@@ -30,6 +30,7 @@ from typing import Dict, Optional
 import torch
 
 from . import lib, ops
+from .trainer import FlatParams
 
 # Philox stream of the row sample.  The dropout masks use offsets layer + step * L, far below this.  G-CRD and GSP share
 # it: a trainer runs one objective.
@@ -71,16 +72,11 @@ class ProjectionHeads:
         self.G_t = z(n, Ftp)
         self.G_t[:, :self.F_t].copy_(teacher_feat.detach().to(torch.float32)[self.train_idx])
 
-        # flat parameters: student W [P, H], b, gamma, beta; teacher W [P, Ft_pad], b, gamma, beta
-        sizes = [P * H, P, P, P, P * Ftp, P, P, P]
-        self.params, self.grads = z(sum(sizes)), z(sum(sizes))
-        self.exp_avg, self.exp_avg_sq = z(sum(sizes)), z(sum(sizes))
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=dev)     # the heads' Adam steps (= BN batches)
+        # flat parameters: student W [P, H], b, gamma, beta; teacher W [P, Ft_pad], b, gamma, beta.  step_count counts the
+        # heads' Adam steps (= BN batches)
+        self.store = FlatParams([(P, H), (P,), (P,), (P,), (P, Ftp), (P,), (P,), (P,)], dev).attach(self)
         self._nbt_base = {"s": 0, "t": 0}         # num_batches_tracked = step_count + base, per head
-        views, off = [], 0
-        for k, shape in zip(sizes, [(P, H), (P,), (P,), (P,), (P, Ftp), (P,), (P,), (P,)]):
-            views.append((self.params[off:off + k].view(shape), self.grads[off:off + k].view(shape)))
-            off += k
+        views = self.store.views
         (self.W_s, self.gW_s), (self.b_s, self.gb_s), (self.gamma_s, self.ggamma_s), (self.beta_s, self.gbeta_s) = views[:4]
         (self.W_t, self.gW_t), (self.b_t, self.gb_t), (self.gamma_t, self.ggamma_t), (self.beta_t, self.gbeta_t) = views[4:]
         self.rm_s, self.rv_s, self.rm_t, self.rv_t = z(P), z(P), z(P), z(P)
@@ -218,13 +214,12 @@ class ProjectionHeads:
         raise NotImplementedError
 
     def optimizer_step(self, lr: float):
-        ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, lr)
+        self.store.adam(lr)
 
     def launches_per_step(self, x, y, train_idx, teacher_logits=None) -> int:
         """b200gnn kernel launches of one whole training step of the bound trainer, the objective included.  Counted by running
         one real step on these inputs: it advances the trainer's and the heads' parameters, Adam state, running statistics and
-        step counters like any other step.  (SAGEStudentTrainer has no counter of its own; GCNStudentTrainer's
-        launches_per_step counts the same step on its captured inputs.)"""
+        step counters like any other step.  (The trainer's own launches_per_step counts the same step on its captured inputs.)"""
         before = lib.launch_count()
         self.trainer._step_impl(x, y, train_idx, teacher_logits)
         return lib.launch_count() - before

@@ -29,6 +29,7 @@ import torch
 from . import lib, ops
 from .hybrid import DensePlan
 from .sparse import SparseTensor, csr_graph_from, device_argsort
+from .trainer import FlatParams, aux_grad
 
 
 def _block_plan(n: int, world: int) -> DensePlan:
@@ -286,42 +287,35 @@ class RGCNTrainer:
             raise lib.B200GnnError("input and hidden widths must be multiples of 4")
 
         # ---- flat parameters: per layer, per node type, WcatT [(1+R_t)·F_in, F_out'] then b [F_out']
-        self._layout = []                          # [layer][type] -> (w_off, kin, nout, b_off)
-        off = 0
+        shapes = []
         for i in range(self.L):
             fi, fo = self.dims_pad[i], self.dims_pad[i + 1]
-            row = []
             for t in range(self.T):
-                kin = (1 + len(self.rels_of[t])) * fi
-                row.append((off, kin, fo, off + kin * fo))
-                off += kin * fo + fo
-            self._layout.append(row)
-        self.n_par = off
-        self.params = torch.zeros(off, device=self.dev)
-        self.grads = torch.zeros(off, device=self.dev)
-        self.exp_avg = torch.zeros(off, device=self.dev)
-        self.exp_avg_sq = torch.zeros(off, device=self.dev)
-        self.step_count = torch.zeros(1, dtype=torch.int32, device=self.dev)
+                shapes += [((1 + len(self.rels_of[t])) * fi, fo), (fo,)]
+        self.store = FlatParams(shapes, self.dev).attach(self)
+        params = iter(p for p, _ in self.store.views)
+        self._wcat, self._b = [], []               # [layer][type] -> view of params
+        for i in range(self.L):
+            row = [(next(params), next(params)) for _ in range(self.T)]
+            self._wcat.append([w for w, _ in row]); self._b.append([b for _, b in row])
         # embedding tables of the types without features, with their Adam moments and the row-head scratch
         self.emb = {t: torch.zeros(n, self.F_in, device=self.dev) for t, n in self.num_nodes.items() if t not in self.x_types}
         self.emb_m = {t: torch.zeros_like(e) for t, e in self.emb.items()}
         self.emb_v = {t: torch.zeros_like(e) for t, e in self.emb.items()}
         self._head = torch.full((max([e.shape[0] for e in self.emb.values()] + [1]),), -1, dtype=torch.int32, device=self.dev)
-        ws = [ops.wgrad_workspace_floats(kin, nout) for row in self._layout for (_, kin, nout, _) in row]
-        self.wgrad_ws = torch.empty(max(ws), device=self.dev)
-        self.loss_out = torch.zeros(3, device=self.dev)
+        self.wgrad_ws = torch.empty(max(ops.wgrad_workspace_floats(*w.shape) for row in self._wcat for w in row), device=self.dev)
         self.reset_parameters(seed)
         self._fwd = None
         self._training = False
 
     # ------------------------------------------------------------------ parameters
     def _wcatT(self, i: int, t: int, buf: Optional[torch.Tensor] = None) -> torch.Tensor:
-        w_off, kin, nout, _ = self._layout[i][t]
-        return (self.params if buf is None else buf)[w_off:w_off + kin * nout].view(kin, nout)
+        w = self._wcat[i][t]
+        return w if buf is None else self.store.like(buf, w)
 
     def _bias(self, i: int, t: int, buf: Optional[torch.Tensor] = None) -> torch.Tensor:
-        _, _, nout, b_off = self._layout[i][t]
-        return (self.params if buf is None else buf)[b_off:b_off + nout]
+        b = self._b[i][t]
+        return b if buf is None else self.store.like(buf, b)
 
     def _blocks(self, i: int, t: int, buf=None):
         """(root weight [F_out, F_in], {relation: weight [F_out, F_in]}, bias [F_out]) as views of the flat buffer."""
@@ -491,11 +485,7 @@ class RGCNTrainer:
         d_logits = self._loss(P, batch, teacher_logits)
         d_feat = None
         if aux is not None:
-            feat = self.out_feat().detach().requires_grad_(True)
-            with torch.enable_grad():
-                loss_aux = aux(feat)
-                (loss_aux * beta).backward()
-            d_feat = feat.grad if feat.grad is not None else torch.zeros_like(feat)
+            d_feat, self.loss_aux = aux_grad(self.out_feat(), aux, beta)
         dx0 = self.backward(d_logits, d_feat)
         if self.emb:
             li = self._fwd["li_int"]
@@ -505,7 +495,6 @@ class RGCNTrainer:
                                    self.step_count, self.lr)
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
         if aux is not None:
-            self.loss_aux = loss_aux.detach()
             self.loss_out[0].add_(self.loss_aux * beta)
         return self.loss_out
 
