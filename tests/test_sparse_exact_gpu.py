@@ -183,6 +183,18 @@ def _nan_flat(n: int) -> torch.Tensor:
     return torch.full((max(n, 1),), NAN_BITS, dtype=torch.int32, device=DEV).view(torch.float32)
 
 
+def _slot_of_row(G: CsrGraph, n_rows: int) -> torch.Tensor:
+    """Fused statistics (SpMM and GAT epilogues): slot s holds the rows of chunks 8s .. 8s+7 minus the hub rows; slot
+    main_grid + h hub row h."""
+    rows = torch.arange(n_rows, device=DEV, dtype=torch.int32)
+    chunk = torch.searchsorted(G.chunk_rowptr, rows, right=True) - 1
+    slot = chunk // 8
+    if G.n_hub:
+        main_grid = (G.n_chunks + 7) // 8
+        slot[G.hub_rows[:G.n_hub].long()] = main_grid + torch.arange(G.n_hub, device=DEV)
+    return slot.long()
+
+
 # ================================================================================================================ plans
 @pytest.mark.parametrize("plan", PLANS, ids=PLAN_IDS)
 @pytest.mark.parametrize("kind", GRAPH_KINDS)
@@ -304,15 +316,7 @@ class SpmmCase:
         return self.Y.view
 
     def slot_of_row(self) -> torch.Tensor:
-        """Fused statistics: slot s holds the rows of chunks 8s .. 8s+7 minus the hub rows; slot main_grid + h hub row h."""
-        G = self.G
-        rows = torch.arange(self.n_rows, device=DEV, dtype=torch.int32)
-        chunk = torch.searchsorted(G.chunk_rowptr, rows, right=True) - 1
-        slot = chunk // 8
-        if G.n_hub:
-            main_grid = (G.n_chunks + 7) // 8
-            slot[G.hub_rows[:G.n_hub].long()] = main_grid + torch.arange(G.n_hub, device=DEV)
-        return slot.long()
+        return _slot_of_row(self.G, self.n_rows)
 
     def check(self, reduce, use_bias, stats, fused, what):
         y = self.run(reduce, use_bias, stats)
