@@ -101,7 +101,9 @@ class PPIGATTrainer:
                  out_channels: int = 121, lr: float = 0.005, seed: int = 0, alpha: float = 0.5, T: float = 1.0,
                  teacher_logits: Optional[Sequence[torch.Tensor]] = None,
                  teacher_feat: Optional[Sequence[torch.Tensor]] = None, dropout: float = 0.0, attn_dropout: float = 0.0,
-                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda"):
+                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda", lsp=None):
+        """lsp: an lsp.PerGraphLSP built for these graphs, run inside every step (and every captured graph): the loss becomes
+        BCE (or kd_criterion) + beta * LSP on the graph's edge list, as ppi_pyg/gnn.py's ``--training lpw``."""
         if dropout != 0.0:
             raise ValueError("dropout > 0 is not implemented (ppi_pyg's GAT baseline class; StudentNet / TeacherNet have none)")
         if attn_dropout != 0.0:
@@ -180,6 +182,12 @@ class PPIGATTrainer:
         self._predict_cache: Dict[tuple, _Graph] = {}
         self._last: Optional[Tuple[_Graph, _Bufs]] = None
         self.epoch = 0
+        self.lsp = lsp
+        if lsp is not None:
+            if self.Dp[-2] != self.Dl[-2]:
+                raise ValueError(f"lsp=: out_feat is stored {self.Dp[-2]} wide per head for a true width of {self.Dl[-2]}; "
+                                 "the LSP kernel reads unpadded rows")
+            lsp.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def _pad_x(self, x: torch.Tensor) -> torch.Tensor:
@@ -301,7 +309,8 @@ class PPIGATTrainer:
                       "gemm_wgrad_tf32x3")
 
     def _backward(self, g: _Graph, b: _Bufs, x: torch.Tensor, d_out_feat: Optional[torch.Tensor] = None):
-        """Consumes the tail's d agg / d res (and optionally d loss / d out_feat); fills self.grads."""
+        """Consumes the tail's d agg / d res (and optionally d loss / d out_feat, copied into b.dA[L-2] unless it is that
+        buffer already); fills self.grads."""
         L_, s = lib.load(), lib.stream_ptr()
         G, Gt, n = g.G, g.Gt, g.n
         for l in range(self.L - 1, -1, -1):
@@ -331,7 +340,7 @@ class PPIGATTrainer:
                                   "transpose_f32")
                 seeded = d_out_feat is not None and l == self.L - 1
                 out = b.dA[l - 1]
-                if seeded:
+                if seeded and d_out_feat is not out:
                     out.copy_(d_out_feat)
                 ops.gemm_tf32x3(gcat, hi, lo, out=out, accumulate=seeded)
             self._ev_fork.record(torch.cuda.current_stream())     # weight gradients only feed Adam: side stream
@@ -357,6 +366,10 @@ class PPIGATTrainer:
             d, loss_aux = aux_grad(self.out_feat(), aux, beta)
             d_feat = torch.zeros(g.n, self.Kout[-2], device=self.device)        # into the stored columns, padding zero
             d_feat[:, self._cols(self.L - 2)] = d
+        elif self.lsp is not None:       # out_feat is A[L-2] unpadded; its gradient is the seed the input-gradient GEMM adds to
+            d_feat = b.dA[self.L - 2]
+            self.lsp.forward_backward(i, b.A[self.L - 2], d_feat, self.loss_out)
+            self.loss_out[2].copy_(self.lsp.loss_aux[0])
         self._backward(g, b, self.x[i], d_out_feat=d_feat)
         self.store.adam(self.lr)
         if aux is not None:
@@ -367,7 +380,9 @@ class PPIGATTrainer:
         """One step on training graph i: BCE, or kd_criterion when teacher logits were given.  ``aux(out_feat)`` (the [n, hidden]
         activation of layer L-2, requires_grad) returns an auxiliary loss that enters as loss + beta * aux and seeds the backward
         at out_feat (gnn.py:213-265); the teacher's out_feat for graph i is ``self.teacher_feat[i]``.  Returns the device tensor
-        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's value when given); no host sync."""
+        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's / the lsp= object's value when given); no host sync."""
+        if aux is not None and self.lsp is not None:
+            raise ValueError("aux= and the trainer's lsp= objective are two auxiliary losses; pass one")
         self._step_impl(i, aux, beta)
         return self.loss_out
 
