@@ -450,9 +450,11 @@ class NceBuffers:
     """Every buffer of one InfoNCE forward + gradient over [Sp, Fp] operands: allocated once, so that a captured step (gcrd.py)
     reuses them on every replay.  g_s / g_t (d loss / d xs, d xt, [Sp, Fp]) exist when requested."""
 
-    def __init__(self, Sp: int, Fp: int, device, need_s: bool = True, need_t: bool = True):
+    def __init__(self, Sp: int, Fp: int, device, need_s: bool = True, need_t: bool = True, alloc=None):
+        """alloc(*shape): where the buffers come from (default torch.empty; gcrd.PerGraphGCRD passes views that several
+        row sets share)."""
         R = nce_chunk_rows(Sp)
-        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=device)
+        e = alloc or (lambda *shape: torch.empty(*shape, dtype=torch.float32, device=device))
         self.Z, self.part, self.loss = e(R, Sp), e(Sp), e(1)
         self.xt_split = (e(Sp, Fp), e(Sp, Fp))                                    # B of Z_c = xs_c · xt^T
         self.g_s = e(Sp, Fp) if need_s else None

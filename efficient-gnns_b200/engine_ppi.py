@@ -23,6 +23,7 @@ stay exactly zero, and state_dict() / out_feat() never show them.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -101,9 +102,11 @@ class PPIGATTrainer:
                  out_channels: int = 121, lr: float = 0.005, seed: int = 0, alpha: float = 0.5, T: float = 1.0,
                  teacher_logits: Optional[Sequence[torch.Tensor]] = None,
                  teacher_feat: Optional[Sequence[torch.Tensor]] = None, dropout: float = 0.0, attn_dropout: float = 0.0,
-                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda", lsp=None):
+                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda", lsp=None, gcrd=None):
         """lsp: an lsp.PerGraphLSP built for these graphs, run inside every step (and every captured graph): the loss becomes
-        BCE (or kd_criterion) + beta * LSP on the graph's edge list, as ppi_pyg/gnn.py's ``--training lpw``."""
+        BCE (or kd_criterion) + beta * LSP on the graph's edge list, as ppi_pyg/gnn.py's ``--training lpw``.  gcrd: a
+        gcrd.PerGraphGCRD built for these graphs, run the same way: BCE (or kd_criterion) + beta * G-CRD through its
+        projection heads, as ``--training nce``; its heads take one Adam step after the model's."""
         if dropout != 0.0:
             raise ValueError("dropout > 0 is not implemented (ppi_pyg's GAT baseline class; StudentNet / TeacherNet have none)")
         if attn_dropout != 0.0:
@@ -129,6 +132,14 @@ class PPIGATTrainer:
         if max(self.Ktot) > 2048 or max(self.Kin) > 2048 or max(self.Hl) > 16:
             raise ValueError("stored layer widths above 2048 or more than 16 heads are not built")
         self.blocks = [[(c, min(WGRAD_BLOCK, k - c)) for c in range(0, k, WGRAD_BLOCK)] for k in self.Ktot]
+        if gcrd is not None:           # refused before any device work
+            if lsp is not None:
+                raise ValueError("gcrd= and lsp= are two auxiliary losses; pass one")
+            if self.Dp[-2] != self.Dl[-2] or self.Kout[-2] > 512:
+                raise ValueError(f"gcrd=: out_feat is stored {self.Kout[-2]} wide for a true width of "
+                                 f"{self.Hl[-2] * self.Dl[-2]}; the student head reads unpadded rows at most 512 wide "
+                                 "(its weight-gradient GEMM)")
+            gcrd.check_graphs([int(x.shape[0]) for x, _, _ in graphs], self.Kout[-2])
 
         # ---- flat parameters, per layer: the column blocks of [W_lin | W_skip] as [in, block] (a weight gradient is one
         # contiguous output), att_l, att_r, a zero vector and b_lin (together the GEMM's bias [0 | b_lin]), b_conv
@@ -182,7 +193,7 @@ class PPIGATTrainer:
         self._predict_cache: Dict[tuple, _Graph] = {}
         self._last: Optional[Tuple[_Graph, _Bufs]] = None
         self.epoch = 0
-        self.lsp = lsp
+        self.lsp, self.gcrd = lsp, gcrd
         if lsp is not None:
             if self.Dp[-2] != self.Dl[-2]:
                 raise ValueError(f"lsp=: out_feat is stored {self.Dp[-2]} wide per head for a true width of {self.Dl[-2]}; "
@@ -356,7 +367,7 @@ class PPIGATTrainer:
     def _teacher(self, i: int) -> Optional[torch.Tensor]:
         return None if self.teacher_logits is None else self.teacher_logits[i]
 
-    def _step_impl(self, i: int, aux=None, beta: float = 1.0):
+    def _step_impl(self, i: int, aux=None, beta: float = 1.0, sample=None):
         g = self.graphs[i]
         b = self.bufs.view(g.n, g.nnz)
         self._forward(g, b, self.x[i], self.y[i], self._teacher(i))
@@ -370,20 +381,31 @@ class PPIGATTrainer:
             d_feat = b.dA[self.L - 2]
             self.lsp.forward_backward(i, b.A[self.L - 2], d_feat, self.loss_out)
             self.loss_out[2].copy_(self.lsp.loss_aux[0])
+        elif self.gcrd is not None:      # the student head's input gradient is stored over all n rows of that seed
+            d_feat = b.dA[self.L - 2]
+            self.gcrd.forward_backward(i, self, b.A[self.L - 2], d_feat, sample)
+            self.loss_out[2].copy_(self.gcrd.loss_aux[0])
         self._backward(g, b, self.x[i], d_out_feat=d_feat)
         self.store.adam(self.lr)
+        if self.gcrd is not None:
+            self.gcrd.optimizer_step(self.lr)
         if aux is not None:
             self.loss_out[0].add_(loss_aux * beta)
             self.loss_out[2].copy_(loss_aux)
 
-    def train_step(self, i: int, aux=None, beta: float = 1.0) -> torch.Tensor:
+    def train_step(self, i: int, aux=None, beta: float = 1.0, sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One step on training graph i: BCE, or kd_criterion when teacher logits were given.  ``aux(out_feat)`` (the [n, hidden]
         activation of layer L-2, requires_grad) returns an auxiliary loss that enters as loss + beta * aux and seeds the backward
         at out_feat (gnn.py:213-265); the teacher's out_feat for graph i is ``self.teacher_feat[i]``.  Returns the device tensor
-        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's / the lsp= object's value when given); no host sync."""
+        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's / the lsp= / gcrd= object's value when given); no host
+        sync.  ``sample`` (positions into graph i's nodes, [S]) replaces the gcrd= object's on-device row draw."""
         if aux is not None and self.lsp is not None:
             raise ValueError("aux= and the trainer's lsp= objective are two auxiliary losses; pass one")
-        self._step_impl(i, aux, beta)
+        if aux is not None and self.gcrd is not None:
+            raise ValueError("aux= and the trainer's gcrd= objective are two auxiliary losses; pass one")
+        if sample is not None and self.gcrd is None:
+            raise ValueError("sample= is the G-CRD row sample; this trainer has no gcrd= objective")
+        self._step_impl(i, aux, beta, sample)
         return self.loss_out
 
     def logits(self) -> torch.Tensor:
@@ -397,9 +419,10 @@ class PPIGATTrainer:
 
     # ------------------------------------------------------------------ CUDA graphs
     def capture(self, warmup: int = 1):
-        """Record one CUDA graph per training graph.  Warm-up steps run on a saved copy of the parameters and Adam state,
-        which is restored afterwards: capturing does not train."""
-        with self.store.preserved():
+        """Record one CUDA graph per training graph.  Warm-up steps run on a saved copy of the parameters and Adam state (and
+        of the gcrd= heads' state), which is restored afterwards: capturing does not train."""
+        heads = self.gcrd.preserved() if self.gcrd is not None else contextlib.nullcontext()
+        with self.store.preserved(), heads:
             for i in range(len(self.graphs)):
                 self._graph[i] = capture_graph(lambda: self._step_impl(i), warmup)
         return self
@@ -407,6 +430,8 @@ class PPIGATTrainer:
     def replay(self, i: int) -> torch.Tensor:
         self._graph[i].replay()
         g = self.graphs[i]
+        if self.gcrd is not None:
+            self.gcrd._last = i
         self._last = (g, self.bufs.view(g.n, g.nnz))
         return self.loss_out
 

@@ -47,27 +47,29 @@ class GSP(ProjectionHeads):
             raise ValueError(f"kernel {kernel!r}: GSP kernels are {sorted(criterion._KERNELS)}")
         super().__init__(teacher_feat, train_idx, hidden, proj_dim, max_samples, beta, seed, bn_eps, bn_momentum)
         self.kernel, self.kernel_id = kernel, criterion._KERNELS[kernel]
-        self.gsp = criterion.GspBuffers(self.Sp, self.P, self.device)
-        # the operands' norms (cosine / poly) or squared norms (l2 / rbf, which the pair pass reads)
-        self.norm_s, self.norm_t = self.gsp.ns, self.gsp.nt
-        self.loss_aux = self.gsp.loss
 
-    def _objective(self, tr):
+    def _objective_buffers(self, r, alloc):
+        r.gsp = criterion.GspBuffers(r.Sp, self.P, self.device)
+        # the operands' norms (cosine / poly) or squared norms (l2 / rbf, which the pair pass reads)
+        r.norm_s, r.norm_t = r.gsp.ns, r.gsp.nt
+        r.loss_aux = r.gsp.loss
+
+    def _objective(self, tr, r):
         L, st = lib.load(), lib.stream_ptr()
-        S, P, k, b = self.S, self.P, self.kernel_id, self.gsp
+        S, P, k, b = r.S, self.P, self.kernel_id, r.gsp
         f = lambda t, name: lib.dptr(t, torch.float32, name)
-        lib.check(L.b200gnn_gsp_operands_f32(self.inds.data_ptr(), S, P, k, f(self.pre_s, "pre_s"), f(self.bn_s, "bn_s"),
-                                             f(self.pre_t, "pre_t"), f(self.bn_t, "bn_t"), _EPS, f(self.x_s, "x_s"),
-                                             f(self.x_t, "x_t"), f(self.norm_s, "norm_s"), f(self.norm_t, "norm_t"), st),
+        lib.check(L.b200gnn_gsp_operands_f32(r.inds.data_ptr(), S, P, k, f(r.pre_s, "pre_s"), f(self.bn_s, "bn_s"),
+                                             f(r.pre_t, "pre_t"), f(self.bn_t, "bn_t"), _EPS, f(r.x_s, "x_s"),
+                                             f(r.x_t, "x_t"), f(r.norm_s, "norm_s"), f(r.norm_t, "norm_t"), st),
                   "gsp_operands_f32")
-        criterion.gsp_chunks(self.x_s, self.x_t, S, k, b)
+        criterion.gsp_chunks(r.x_s, r.x_t, S, k, b)
         # backward: dz = beta * d loss / d BN output at the sampled rows, zero elsewhere; BatchNorm backward over all rows
-        self.dz_s.zero_()
-        self.dz_t.zero_()
-        lib.check(L.b200gnn_gsp_backward_f32(self.inds.data_ptr(), S, P, k, f(b.g_s, "g_s"), f(b.g_t, "g_t"), f(self.x_s, "x_s"),
-                                             f(self.x_t, "x_t"), f(self.norm_s, "norm_s"), f(self.norm_t, "norm_t"),
-                                             f(b.rc_s, "rc_s"), f(b.rc_t, "rc_t"), _EPS, f(self.pre_s, "pre_s"),
-                                             f(self.bn_s, "bn_s"), f(self.pre_t, "pre_t"), f(self.bn_t, "bn_t"), self.beta,
-                                             f(self.dz_s, "dz_s"), f(self.dz_t, "dz_t"), f(self.bpart_s, "part_s"),
-                                             f(self.bpart_t, "part_t"), f(self.loss_aux, "loss_aux"),
+        r.dz_s.zero_()
+        r.dz_t.zero_()
+        lib.check(L.b200gnn_gsp_backward_f32(r.inds.data_ptr(), S, P, k, f(b.g_s, "g_s"), f(b.g_t, "g_t"), f(r.x_s, "x_s"),
+                                             f(r.x_t, "x_t"), f(r.norm_s, "norm_s"), f(r.norm_t, "norm_t"),
+                                             f(b.rc_s, "rc_s"), f(b.rc_t, "rc_t"), _EPS, f(r.pre_s, "pre_s"),
+                                             f(self.bn_s, "bn_s"), f(r.pre_t, "pre_t"), f(self.bn_t, "bn_t"), self.beta,
+                                             f(r.dz_s, "dz_s"), f(r.dz_t, "dz_t"), f(self.bpart_s, "part_s"),
+                                             f(self.bpart_t, "part_t"), f(r.loss_aux, "loss_aux"),
                                              f(tr.loss_out, "loss_out"), st), "gsp_backward_f32")
