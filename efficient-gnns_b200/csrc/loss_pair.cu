@@ -32,6 +32,38 @@ __device__ __forceinline__ void block_sum_store(float v, float* partial) {
   }
 }
 
+// ---------------------------------------------------------------- row helpers
+// Shared by the row passes below and the GSP rows passes, so that a fused pass computes what the eager sequence of
+// row_normalize / row_sqnorm / row_axpy computes, bit for bit.  A warp owns a row; lane l visits columns l, l + 32, ...
+
+// sum_k x[k]^2 of one row: each lane's columns in order, then the warp's butterfly
+__device__ __forceinline__ float row_sumsq(const float* __restrict__ xr, int F, int lane) {
+  float ss = 0.f;
+  for (int k = lane; k < F; k += 32) { const float v = xr[k]; ss = fmaf(v, v, ss); }
+  return warp_sum_f(ss);
+}
+// o = xr * scale / max(||xr||, eps); returns ||xr||
+__device__ __forceinline__ float normalize_row(const float* __restrict__ xr, int F, float eps, float scale, float* __restrict__ o,
+                                               int lane) {
+  const float nrm = sqrtf(row_sumsq(xr, F, lane));
+  const float inv = scale / fmaxf(nrm, eps);
+  for (int k = lane; k < F; k += 32) o[k] = xr[k] * inv;
+  return nrm;
+}
+// u . d_out of the normalise backward (u = out / scale); d(k) loads d_out[k]
+template <class D>
+__device__ __forceinline__ float normalize_bwd_dot(const float* __restrict__ o, D d, int F, float inv_scale, int lane) {
+  float dot = 0.f;
+  for (int k = lane; k < F; k += 32) dot = fmaf(o[k] * inv_scale, d(k), dot);
+  return warp_sum_f(dot);
+}
+// one element of the normalise backward: inv = scale / max(norm, eps), clamped = norm < eps
+__device__ __forceinline__ float normalize_bwd_elem(float o, float d, float inv_scale, float dot, float inv, bool clamped) {
+  return clamped ? d * inv : inv * (d - o * inv_scale * dot);
+}
+// y + alpha * coef * x (row_axpy's element)
+__device__ __forceinline__ float axpy_elem(float alpha, float coef, float x, float y) { return fmaf(alpha * coef, x, y); }
+
 // ---------------------------------------------------------------- F.normalize(x, p=2, dim=-1)  (eps = 1e-12)
 // warp per row; out = x / max(||x||, eps); norm_out[row] = ||x||
 __global__ void __launch_bounds__(256) row_normalize_fwd_kernel(const float* __restrict__ x, int64_t n, int F, float eps,
@@ -39,14 +71,7 @@ __global__ void __launch_bounds__(256) row_normalize_fwd_kernel(const float* __r
                                                                 float* __restrict__ norm_out) {
   const int lane = threadIdx.x & 31;
   for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n; r += (int64_t)gridDim.x * 8) {
-    const float* xr = x + (size_t)r * F;
-    float ss = 0.f;
-    for (int k = lane; k < F; k += 32) { const float v = xr[k]; ss = fmaf(v, v, ss); }
-    ss = warp_sum_f(ss);
-    const float nrm = sqrtf(ss);
-    const float inv = scale / fmaxf(nrm, eps);
-    float* o = out + (size_t)r * F;
-    for (int k = lane; k < F; k += 32) o[k] = xr[k] * inv;
+    const float nrm = normalize_row(x + (size_t)r * F, F, eps, scale, out + (size_t)r * F, lane);
     if (lane == 0 && norm_out) norm_out[r] = nrm;
   }
 }
@@ -61,15 +86,13 @@ __global__ void __launch_bounds__(256) row_normalize_bwd_kernel(const float* __r
   for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n; r += (int64_t)gridDim.x * 8) {
     const float* o = out + (size_t)r * F;
     const float* g = d_out + (size_t)r * F;
-    float dot = 0.f;
-    for (int k = lane; k < F; k += 32) dot = fmaf(o[k] * inv_scale, g[k], dot);
-    dot = warp_sum_f(dot);
+    const float dot = normalize_bwd_dot(o, [g](int k) { return g[k]; }, F, inv_scale, lane);
     const float nrm = norm[r];
     const bool clamped = nrm < eps;
     const float inv = scale / fmaxf(nrm, eps);
     float* dx = d_x + (size_t)r * F;
     for (int k = lane; k < F; k += 32) {
-      const float v = clamped ? g[k] * inv : inv * (g[k] - o[k] * inv_scale * dot);
+      const float v = normalize_bwd_elem(o[k], g[k], inv_scale, dot, inv, clamped);
       dx[k] = accumulate ? dx[k] + v : v;
     }
   }
@@ -92,10 +115,7 @@ __global__ void __launch_bounds__(256) mse_fwd_bwd_kernel(const float* __restric
 __global__ void __launch_bounds__(256) row_sqnorm_kernel(const float* __restrict__ x, int64_t n, int F, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n; r += (int64_t)gridDim.x * 8) {
-    const float* xr = x + (size_t)r * F;
-    float ss = 0.f;
-    for (int k = lane; k < F; k += 32) { const float v = xr[k]; ss = fmaf(v, v, ss); }
-    ss = warp_sum_f(ss);
+    const float ss = row_sumsq(x + (size_t)r * F, F, lane);
     if (lane == 0) out[r] = ss;
   }
 }
@@ -168,6 +188,33 @@ __global__ void __launch_bounds__(256) transpose_kernel(const float* __restrict_
 // are set to zero (so a GEMM may contract over the padded pitch).  BOTH: Gt <- d loss / d Gt in the same pass, with the
 // teacher's own coefficient sums in rc_t; its expressions are the student's with the roles of the two sides swapped, so
 // the result is that of a second one-sided pass on (Gt, Gs, nt, ns).
+//
+// The similarity of one pair, shared by the pair passes and the similarity builder: from the Gram entry G_ij and (l2 / rbf)
+// the squared norms n_i, n[j] (read only for l2 / rbf), sim and its derivatives d sim / d G_ij and d sim / d n_i
+// (= d / d n_j).  diag: i == j, whose l2 / rbf distance is exactly 0 whatever rounding left in n_i + n_j - 2 G_ii.
+struct PairSim {
+  float sim, d_g, d_n;
+};
+__device__ __forceinline__ PairSim gsp_sim(int kernel, float g, float ni, const float* __restrict__ n, int j, bool diag) {
+  PairSim p;
+  p.d_n = 0.f;
+  if (kernel == 0) { p.sim = g; p.d_g = 1.f; }
+  else if (kernel == 1) { p.sim = g * g; p.d_g = 2.f * g; }
+  else {
+    float d2 = fmaxf(ni + n[j] - 2.f * g, 0.f);
+    if (diag) d2 = 0.f;
+    if (kernel == 2) {
+      p.sim = sqrtf(d2);
+      const float inv = p.sim > 0.f ? 0.5f / p.sim : 0.f;   // d sqrt(d2)/d d2, sub-gradient 0 at 0 (torch .norm backward)
+      p.d_g = -2.f * inv; p.d_n = inv;
+    } else {
+      p.sim = expf(-0.5f * d2);
+      p.d_g = p.sim; p.d_n = -0.5f * p.sim;
+    }
+  }
+  return p;
+}
+
 template <bool BOTH>
 __global__ void __launch_bounds__(256) gsp_pair_kernel(float* __restrict__ Gs, float* __restrict__ Gt, int64_t ld, int S,
                                                        int row0, const float* __restrict__ ns, const float* __restrict__ nt,
@@ -180,35 +227,17 @@ __global__ void __launch_bounds__(256) gsp_pair_kernel(float* __restrict__ Gs, f
   float acc = 0.f, rs = 0.f, rt = 0.f;
   const float nsi = (kernel >= 2) ? ns[row] : 0.f, nti = (kernel >= 2) ? nt[row] : 0.f;
   for (int j = threadIdx.x; j < S; j += blockDim.x) {
-    float ss, st, ds_dg, dt_dg, ds_dn = 0.f, dt_dn = 0.f;   // d sim / d G_ij , d sim / d n_i (= d/d n_j), per side
-    const float a = gs[j], b = gt[j];
-    if (kernel == 0) { ss = a; st = b; ds_dg = 1.f; dt_dg = 1.f; }
-    else if (kernel == 1) { ss = a * a; st = b * b; ds_dg = 2.f * a; dt_dg = 2.f * b; }
-    else {
-      float d2s = fmaxf(nsi + ns[j] - 2.f * a, 0.f), d2t = fmaxf(nti + nt[j] - 2.f * b, 0.f);
-      if (j == row) { d2s = 0.f; d2t = 0.f; }
-      if (kernel == 2) {
-        ss = sqrtf(d2s); st = sqrtf(d2t);
-        const float inv_s = ss > 0.f ? 0.5f / ss : 0.f;   // d sqrt(d2)/d d2, sub-gradient 0 at 0 (torch .norm backward)
-        const float inv_t = st > 0.f ? 0.5f / st : 0.f;
-        ds_dg = -2.f * inv_s; ds_dn = inv_s;
-        dt_dg = -2.f * inv_t; dt_dn = inv_t;
-      } else {
-        ss = expf(-0.5f * d2s); st = expf(-0.5f * d2t);
-        ds_dg = ss; ds_dn = -0.5f * ss;
-        dt_dg = st; dt_dn = -0.5f * st;
-      }
-    }
-    const float diff = ss - st;
+    const PairSim s = gsp_sim(kernel, gs[j], nsi, ns, j, j == row), t = gsp_sim(kernel, gt[j], nti, nt, j, j == row);
+    const float diff = s.sim - t.sim;
     acc = fmaf(diff, diff, acc);
     const float g = w * diff;                 // d loss / d sim_s
-    gs[j] = g * ds_dg;
-    rs += g * ds_dn;
+    gs[j] = g * s.d_g;
+    rs += g * s.d_n;
     if (BOTH) {
-      const float diff_t = st - ss;
+      const float diff_t = t.sim - s.sim;
       const float g_t = w * diff_t;           // d loss / d sim_t
-      gt[j] = g_t * dt_dg;
-      rt += g_t * dt_dn;
+      gt[j] = g_t * t.d_g;
+      rt += g_t * t.d_n;
     }
   }
   for (int64_t j = (int64_t)S + threadIdx.x; j < ld; j += blockDim.x) {
@@ -239,7 +268,106 @@ __global__ void __launch_bounds__(256) row_axpy_kernel(const float* __restrict__
                                                        int F, float alpha, float* __restrict__ y) {
   const int64_t total = n * (int64_t)F;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
-    y[i] = fmaf(alpha * coef[i / F], x[i], y[i]);
+    y[i] = axpy_elem(alpha, coef[i / F], x[i], y[i]);
+}
+
+// ---------------------------------------------------------------- GSP against a fixed teacher (PPI: gpw on out_feat)
+// The teacher of the PPI step is frozen, so its similarities are built once per graph: sim[r][j] = k(G[r][j]) for rows
+// [row0, row0 + gridDim.x) of the n x n teacher Gram matrix (G and sim point at the chunk's first row).
+__global__ void __launch_bounds__(256) gsp_sim_kernel(const float* __restrict__ G, int64_t ldg, int n, int row0,
+                                                      const float* __restrict__ sq, int kernel, float* __restrict__ sim,
+                                                      int64_t lds) {
+  const int row = row0 + blockIdx.x;
+  const float* g = G + (size_t)blockIdx.x * ldg;
+  float* s = sim + (size_t)blockIdx.x * lds;
+  const float ni = kernel >= 2 ? sq[row] : 0.f;
+  for (int j = threadIdx.x; j < n; j += blockDim.x) s[j] = gsp_sim(kernel, g[j], ni, sq, j, j == row).sim;
+}
+
+// gsp_pair_kernel<false> with the teacher's similarity read from the stored sim_t instead of formed from its Gram chunk:
+// sample position i is node inds[i] (inds null: the identity), so sim_t is read at [inds[row]][inds[j]] while the l2 / rbf
+// diagonal and every stored row are sample positions.
+__global__ void __launch_bounds__(256) gsp_pair_fixed_kernel(float* __restrict__ Gs, int64_t ld, int S, int row0,
+                                                             const float* __restrict__ ns, const float* __restrict__ sim_t,
+                                                             int64_t ldt, const int32_t* __restrict__ inds, int kernel,
+                                                             float w /* 2 / S^2 */, float* __restrict__ rc_s,
+                                                             float* __restrict__ partial) {
+  __shared__ float s_red[32];
+  const int row = row0 + blockIdx.x;
+  float* gs = Gs + (size_t)blockIdx.x * ld;
+  const float* st = sim_t + (size_t)(inds ? __ldg(inds + row) : row) * ldt;
+  float acc = 0.f, rs = 0.f;
+  const float nsi = (kernel >= 2) ? ns[row] : 0.f;
+  for (int j = threadIdx.x; j < S; j += blockDim.x) {
+    const PairSim s = gsp_sim(kernel, gs[j], nsi, ns, j, j == row);
+    const float diff = s.sim - st[inds ? __ldg(inds + j) : j];
+    acc = fmaf(diff, diff, acc);
+    const float g = w * diff;                 // d loss / d sim_s
+    gs[j] = g * s.d_g;
+    rs += g * s.d_n;
+  }
+  for (int64_t j = (int64_t)S + threadIdx.x; j < ld; j += blockDim.x) gs[j] = 0.f;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  acc = warp_sum_f(acc); rs = warp_sum_f(rs);
+  if (lane == 0) s_red[warp] = acc;
+  __syncthreads();
+  if (warp == 0) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) partial[row] = t; }
+  __syncthreads();
+  if (lane == 0) s_red[warp] = rs;
+  __syncthreads();
+  if (warp == 0 && rc_s) { float t = lane < nw ? s_red[lane] : 0.f; t = warp_sum_f(t); if (lane == 0) rc_s[row] = t; }
+}
+
+// The operands of the fixed-teacher pair pass, straight from feature rows (no heads): x[j] = feat[inds[j]] normalised with
+// F.normalize's eps and norm[j] = its norm (cosine / poly), or copied with norm[j] = its squared norm (l2 / rbf).  A warp
+// per row, the arithmetic of row_normalize_fwd / row_sqnorm.
+__global__ void __launch_bounds__(256) gsp_rows_operands_kernel(const float* __restrict__ feat, int64_t ldf,
+                                                                const int32_t* __restrict__ inds, int64_t S, int F, int raw,
+                                                                float eps, float* __restrict__ x, int64_t ldx,
+                                                                float* __restrict__ norm) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t j = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); j < S; j += (int64_t)gridDim.x * 8) {
+    const float* xr = feat + (size_t)(inds ? __ldg(inds + j) : j) * ldf;
+    float* o = x + (size_t)j * ldx;
+    float v;
+    if (raw) {
+      v = row_sumsq(xr, F, lane);
+      for (int k = lane; k < F; k += 32) o[k] = xr[k];
+    } else {
+      v = normalize_row(xr, F, eps, 1.f, o, lane);
+    }
+    if (lane == 0) norm[j] = v;
+  }
+}
+
+// The way back from g = dG . x (the chunk loop's product) to beta * d loss / d feat, stored to row inds[j] of d_feat:
+// d = 2 g through the normalise backward (cosine / poly), or 2 g + 4 rc[j] x (l2 / rbf), then times beta; the
+// arithmetic of the eager row_normalize_bwd / row_axpy and the autograd multiply by beta.  loss_total[0] += beta *
+// loss_aux[0] as two roundings, as the eager loss[0].add_(loss_aux * beta).
+__global__ void __launch_bounds__(256) gsp_rows_backward_kernel(const int32_t* __restrict__ inds, int64_t S, int F, int raw,
+                                                                const float* __restrict__ g, const float* __restrict__ x,
+                                                                int64_t ldx, const float* __restrict__ norm,
+                                                                const float* __restrict__ rc, float eps, float beta,
+                                                                float* __restrict__ d_feat, int64_t ldd,
+                                                                const float* __restrict__ loss_aux,
+                                                                float* __restrict__ loss_total) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t j = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); j < S; j += (int64_t)gridDim.x * 8) {
+    const float* gj = g + (size_t)j * ldx;
+    const float* o = x + (size_t)j * ldx;
+    float* d = d_feat + (size_t)(inds ? __ldg(inds + j) : j) * ldd;
+    if (raw) {
+      const float c = rc[j];
+      for (int k = lane; k < F; k += 32) d[k] = axpy_elem(4.f, c, o[k], 2.f * gj[k]) * beta;
+    } else {
+      const float dot = normalize_bwd_dot(o, [gj](int k) { return 2.f * gj[k]; }, F, 1.f, lane);
+      const float nrm = norm[j];
+      const bool clamped = nrm < eps;
+      const float inv = 1.f / fmaxf(nrm, eps);
+      for (int k = lane; k < F; k += 32) d[k] = normalize_bwd_elem(o[k], 2.f * gj[k], 1.f, dot, inv, clamped) * beta;
+    }
+  }
+  if (loss_total && blockIdx.x == 0 && threadIdx.x == 0) loss_total[0] = __fadd_rn(loss_total[0], __fmul_rn(loss_aux[0], beta));
 }
 
 // F.binary_cross_entropy_with_logits(z, t) (ppi_pyg/criterion.py:11,13): element loss max(z,0) - z t + log1p(exp(-|z|)),
@@ -419,5 +547,71 @@ extern "C" int b200gnn_row_axpy_f32(const float* x, const float* coef, int64_t n
   if (!x || !coef || !y || n < 0 || F <= 0) return B200GNN_ERR_BAD_ARG;
   if (n == 0) return B200GNN_OK;
   row_axpy_kernel<<<ew_grid(n * F), 256, 0, (cudaStream_t)stream>>>(x, coef, n, (int)F, alpha, y);
+  return check_launch();
+}
+
+// ---------------------------------------------------------------- GSP against a fixed teacher
+static inline bool f32_aligned(const void* p) { return aligned_to(p, 4); }
+
+// sim = rows [row_offset, row_offset + n_rows) of the n x n similarity matrix from the same rows of the Gram matrix
+// (G at pitch ldg >= n, sim at pitch ld_sim >= n, both pointing at the chunk's first row); sq[n]: squared norms (l2 / rbf).
+extern "C" int b200gnn_gsp_sim_chunk_f32(const float* G, int64_t ldg, int64_t n_rows, int64_t n, int64_t row_offset,
+                                         const float* sq, int kernel, float* sim, int64_t ld_sim, void* stream) {
+  if (!G || !sim || n <= 0 || n >= INT32_MAX || ldg < n || ld_sim < n || n_rows <= 0 || row_offset < 0 ||
+      row_offset + n_rows > n || kernel < 0 || kernel > 3 || (kernel >= 2 && !sq))
+    return B200GNN_ERR_BAD_ARG;
+  if (!f32_aligned(G) || !f32_aligned(sim) || (sq && !f32_aligned(sq))) return B200GNN_ERR_BAD_ARG;
+  gsp_sim_kernel<<<(int)n_rows, 256, 0, (cudaStream_t)stream>>>(G, ldg, (int)n, (int)row_offset, sq, kernel, sim, ld_sim);
+  return check_launch();
+}
+
+// The student side of b200gnn_gsp_pair_chunk_f32 against a stored teacher similarity matrix sim_t [n_t, n_t] (pitch
+// ld_t): Gs = rows [row_offset, row_offset + n_rows) of the S x S student Gram matrix at pitch ld >= S, overwritten by
+// d loss / d Gs, columns S..ld-1 zeroed; partial[S] and (l2 / rbf) rc_s[S] at the sample rows.  inds[S] (nullable: the
+// identity, S <= n_t) maps sample positions to rows of sim_t.
+extern "C" int b200gnn_gsp_pair_fixed_chunk_f32(float* Gs, int64_t ld, int64_t n_rows, int64_t S, int64_t row_offset,
+                                                const float* ns, const float* sim_t, int64_t ld_t, int64_t n_t,
+                                                const int32_t* inds, int kernel, float* rc_s, float* partial, void* stream) {
+  if (!Gs || !sim_t || !partial || S <= 0 || S >= INT32_MAX || ld < S || n_rows <= 0 || row_offset < 0 ||
+      row_offset + n_rows > S || n_t <= 0 || ld_t < n_t || S > n_t || kernel < 0 || kernel > 3)
+    return B200GNN_ERR_BAD_ARG;
+  if (kernel >= 2 && (!ns || !rc_s)) return B200GNN_ERR_BAD_ARG;
+  const void* al[] = {Gs, sim_t, partial, ns, rc_s, inds};
+  for (const void* p : al)
+    if (p && !f32_aligned(p)) return B200GNN_ERR_BAD_ARG;
+  const double n2 = (double)S * (double)S;
+  gsp_pair_fixed_kernel<<<(int)n_rows, 256, 0, (cudaStream_t)stream>>>(Gs, ld, (int)S, (int)row_offset, ns, sim_t, ld_t, inds,
+                                                                      kernel, (float)(2.0 / n2), rc_s, partial);
+  return check_launch();
+}
+
+// x[j] (pitch ldx) and norm[j] of feat row inds[j] (inds nullable: row j), feat at pitch ldf.
+extern "C" int b200gnn_gsp_rows_operands_f32(const float* feat, int64_t ldf, const int32_t* inds, int64_t S, int64_t F,
+                                             int kernel, float eps, float* x, int64_t ldx, float* norm, void* stream) {
+  if (!feat || !x || !norm || S <= 0 || S >= INT32_MAX || F <= 0 || F > B200GNN_GSP_ROWS_MAX_F || ldf < F || ldx < F ||
+      kernel < 0 || kernel > 3 || !(eps > 0.f))
+    return B200GNN_ERR_BAD_ARG;
+  const void* al[] = {feat, x, norm, inds};
+  for (const void* p : al)
+    if (p && !f32_aligned(p)) return B200GNN_ERR_BAD_ARG;
+  gsp_rows_operands_kernel<<<ew_grid(S, 8), 256, 0, (cudaStream_t)stream>>>(feat, ldf, inds, S, (int)F, kernel >= 2, eps, x,
+                                                                           ldx, norm);
+  return check_launch();
+}
+
+// d_feat[inds[j]] (pitch ldd; inds nullable: row j) = beta * the operand gradient of x[j] from g[j] = (dG . x)[j];
+// norm (cosine / poly) or rc (l2 / rbf) required.  loss_total[0] += beta * loss_aux[0] when loss_total is given.
+extern "C" int b200gnn_gsp_rows_backward_f32(const int32_t* inds, int64_t S, int64_t F, int kernel, const float* g,
+                                             const float* x, int64_t ldx, const float* norm, const float* rc, float eps,
+                                             float beta, float* d_feat, int64_t ldd, const float* loss_aux,
+                                             float* loss_total, void* stream) {
+  if (!g || !x || !d_feat || S <= 0 || S >= INT32_MAX || F <= 0 || F > B200GNN_GSP_ROWS_MAX_F || ldx < F || ldd < F ||
+      kernel < 0 || kernel > 3 || !(eps > 0.f) || (kernel >= 2 ? !rc : !norm) || (loss_total && !loss_aux))
+    return B200GNN_ERR_BAD_ARG;
+  const void* al[] = {inds, g, x, norm, rc, d_feat, loss_aux, loss_total};
+  for (const void* p : al)
+    if (p && !f32_aligned(p)) return B200GNN_ERR_BAD_ARG;
+  gsp_rows_backward_kernel<<<ew_grid(S, 8), 256, 0, (cudaStream_t)stream>>>(inds, S, (int)F, kernel >= 2, g, x, ldx, norm, rc,
+                                                                           eps, beta, d_feat, ldd, loss_aux, loss_total);
   return check_launch();
 }

@@ -102,11 +102,13 @@ class PPIGATTrainer:
                  out_channels: int = 121, lr: float = 0.005, seed: int = 0, alpha: float = 0.5, T: float = 1.0,
                  teacher_logits: Optional[Sequence[torch.Tensor]] = None,
                  teacher_feat: Optional[Sequence[torch.Tensor]] = None, dropout: float = 0.0, attn_dropout: float = 0.0,
-                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda", lsp=None, gcrd=None):
+                 weight_decay: float = 0.0, negative_slope: float = 0.2, device="cuda", lsp=None, gcrd=None, gsp=None):
         """lsp: an lsp.PerGraphLSP built for these graphs, run inside every step (and every captured graph): the loss becomes
         BCE (or kd_criterion) + beta * LSP on the graph's edge list, as ppi_pyg/gnn.py's ``--training lpw``.  gcrd: a
         gcrd.PerGraphGCRD built for these graphs, run the same way: BCE (or kd_criterion) + beta * G-CRD through its
-        projection heads, as ``--training nce``; its heads take one Adam step after the model's."""
+        projection heads, as ``--training nce``; its heads take one Adam step after the model's.  gsp: a gsp.PerGraphGSP
+        built for these graphs, run the same way: BCE (or kd_criterion) + beta * GSP between out_feat and the teacher's
+        out_feat, as ``--training gpw``."""
         if dropout != 0.0:
             raise ValueError("dropout > 0 is not implemented (ppi_pyg's GAT baseline class; StudentNet / TeacherNet have none)")
         if attn_dropout != 0.0:
@@ -140,6 +142,13 @@ class PPIGATTrainer:
                                  f"{self.Hl[-2] * self.Dl[-2]}; the student head reads unpadded rows at most 512 wide "
                                  "(its weight-gradient GEMM)")
             gcrd.check_graphs([int(x.shape[0]) for x, _, _ in graphs], self.Kout[-2])
+        if gsp is not None:
+            if lsp is not None or gcrd is not None:
+                raise ValueError("gsp= and lsp= / gcrd= are two auxiliary losses; pass one")
+            if self.Dp[-2] != self.Dl[-2]:
+                raise ValueError(f"gsp=: out_feat is stored {self.Dp[-2]} wide per head for a true width of {self.Dl[-2]}; "
+                                 "the GSP row passes read unpadded rows")
+            gsp.check_graphs([int(x.shape[0]) for x, _, _ in graphs], self.Kout[-2])
 
         # ---- flat parameters, per layer: the column blocks of [W_lin | W_skip] as [in, block] (a weight gradient is one
         # contiguous output), att_l, att_r, a zero vector and b_lin (together the GEMM's bias [0 | b_lin]), b_conv
@@ -193,7 +202,7 @@ class PPIGATTrainer:
         self._predict_cache: Dict[tuple, _Graph] = {}
         self._last: Optional[Tuple[_Graph, _Bufs]] = None
         self.epoch = 0
-        self.lsp, self.gcrd = lsp, gcrd
+        self.lsp, self.gcrd, self.gsp = lsp, gcrd, gsp
         if lsp is not None:
             if self.Dp[-2] != self.Dl[-2]:
                 raise ValueError(f"lsp=: out_feat is stored {self.Dp[-2]} wide per head for a true width of {self.Dl[-2]}; "
@@ -385,6 +394,10 @@ class PPIGATTrainer:
             d_feat = b.dA[self.L - 2]
             self.gcrd.forward_backward(i, self, b.A[self.L - 2], d_feat, sample)
             self.loss_out[2].copy_(self.gcrd.loss_aux[0])
+        elif self.gsp is not None:       # beta * d loss / d out_feat is stored straight into that seed
+            d_feat = b.dA[self.L - 2]
+            self.gsp.forward_backward(i, self, b.A[self.L - 2], d_feat, sample)
+            self.loss_out[2].copy_(self.gsp.loss_aux[0])
         self._backward(g, b, self.x[i], d_out_feat=d_feat)
         self.store.adam(self.lr)
         if self.gcrd is not None:
@@ -397,14 +410,19 @@ class PPIGATTrainer:
         """One step on training graph i: BCE, or kd_criterion when teacher logits were given.  ``aux(out_feat)`` (the [n, hidden]
         activation of layer L-2, requires_grad) returns an auxiliary loss that enters as loss + beta * aux and seeds the backward
         at out_feat (gnn.py:213-265); the teacher's out_feat for graph i is ``self.teacher_feat[i]``.  Returns the device tensor
-        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's / the lsp= / gcrd= object's value when given); no host
-        sync.  ``sample`` (positions into graph i's nodes, [S]) replaces the gcrd= object's on-device row draw."""
+        [loss, loss_cls, loss_aux] (loss_aux: the kd term, or aux's / the lsp= / gcrd= / gsp= object's value when given); no
+        host sync.  ``sample`` (positions into graph i's nodes, [S]) replaces the gcrd= or gsp= object's on-device row
+        draw."""
         if aux is not None and self.lsp is not None:
             raise ValueError("aux= and the trainer's lsp= objective are two auxiliary losses; pass one")
         if aux is not None and self.gcrd is not None:
             raise ValueError("aux= and the trainer's gcrd= objective are two auxiliary losses; pass one")
-        if sample is not None and self.gcrd is None:
+        if aux is not None and self.gsp is not None:
+            raise ValueError("aux= and the trainer's gsp= objective are two auxiliary losses; pass one")
+        if sample is not None and self.gcrd is None and self.gsp is None:
             raise ValueError("sample= is the G-CRD row sample; this trainer has no gcrd= objective")
+        if sample is not None and self.gsp is not None:
+            self.gsp.check_sample(i, sample)
         self._step_impl(i, aux, beta, sample)
         return self.loss_out
 
@@ -432,6 +450,8 @@ class PPIGATTrainer:
         g = self.graphs[i]
         if self.gcrd is not None:
             self.gcrd._last = i
+        if self.gsp is not None:
+            self.gsp._last = i
         self._last = (g, self.bufs.view(g.n, g.nnz))
         return self.loss_out
 

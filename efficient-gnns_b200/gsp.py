@@ -22,13 +22,18 @@ from inside their step, so ``capture()`` / ``replay()`` run it in the same CUDA 
 
 The row sample is G-CRD's (same sampler and Philox stream; a trainer runs one objective); ``train_step(..., sample=)``
 injects one.
+
+``PerGraphGSP`` is GSP for engine_ppi's PPI student, which has no heads: the loss compares the student's out_feat with the
+frozen teacher's, so each graph's teacher similarities are constants built once.
 """
 from __future__ import annotations
 
+from typing import List, Optional, Sequence
+
 import torch
 
-from . import criterion, lib
-from .heads import ProjectionHeads
+from . import criterion, lib, ops
+from .heads import ProjectionHeads, _ceil4, _Pool, draw_sample
 
 _EPS = 1e-12                                      # F.normalize
 
@@ -73,3 +78,190 @@ class GSP(ProjectionHeads):
                                              f(r.dz_s, "dz_s"), f(r.dz_t, "dz_t"), f(self.bpart_s, "part_s"),
                                              f(self.bpart_t, "part_t"), f(r.loss_aux, "loss_aux"),
                                              f(tr.loss_out, "loss_out"), st), "gsp_backward_f32")
+
+
+class _GraphGSP:
+    """One training graph's share of PerGraphGSP: n, S = min(max_samples, n), Sp, its sample, its teacher similarities
+    sim_t [n, n] (a view of the object's flat allocation) and its views of the per-step buffers, at the geometry the eager
+    gpw_criterion gives S rows: operands [Sp, H], Gram chunks of gsp_chunk_rows(Sp) rows at pitch Sp."""
+
+    def __init__(self, n: int, S: int, sim_t: torch.Tensor, x_s: torch.Tensor, H: int, device, alloc):
+        self.n, self.S, self.Sp, self.sim_t, self.x_s = n, S, _ceil4(S), sim_t, x_s
+        Sp = self.Sp
+        self.perm = torch.arange(n, dtype=torch.int32, device=device)
+        self.inds = self.perm[:S]
+        self.G = alloc(criterion.gsp_chunk_rows(Sp), Sp)
+        self.split, self.splitT = (alloc(Sp, H), alloc(Sp, H)), (alloc(H, Sp), alloc(H, Sp))
+        self.g = alloc(Sp, H)                                   # dG . x
+        self.norm, self.rc, self.part = alloc(Sp), alloc(Sp), alloc(Sp)
+        self.loss_aux = alloc(1)
+
+
+class PerGraphGSP:
+    """GSP inside engine_ppi's captured step: the reference's PPI ``train()`` with ``--training gpw`` (ppi_pyg/gnn.py:230-239;
+    criterion.py:54-89) applies ``gpw_criterion(out, labels, model.out_feat, teacher_model.out_feat, kernel, beta,
+    max_samples)`` to each training graph, every node a row and no projection heads: BCE (or kd_criterion) + beta * mean((sim_s
+    - sim_t)^2) over S = min(max_samples, n) rows.
+
+    The teacher runs in eval mode with frozen parameters, so each graph's teacher similarity matrix is a constant: it is
+    built once, at construction, with the eager path's kernels and shapes (normalise or squared norms, the 3xTF32 Gram at
+    pitch Sp and K = F_t in row chunks, b200gnn_gsp_sim_chunk_f32), and kept as an [n, n] view of one flat allocation
+    (``sim_bytes`` in all).  A GEMM row does not depend on the M tiling and these GEMMs have no split-K, so sim_t equals the
+    teacher similarities the eager path forms, and the step never touches the 1024-wide teacher features again.  On graph
+    i the step runs, as launches only (capturable):
+
+        sample       only when S < n: G-CRD's sampler at (trainer seed, SAMPLE_STREAM, device step counter)
+        operands     b200gnn_gsp_rows_operands_f32: the S rows of out_feat normalised (cosine / poly) or copied with their
+                     squared norms (l2 / rbf), zero-padded to [Sp, H]
+        loss         the student side of criterion.gsp_chunks: both splits of the operands, then per chunk the Gram GEMM,
+                     b200gnn_gsp_pair_fixed_chunk_f32 against sim_t, and dG . x; b200gnn_gsp_finish_f32
+        backward     b200gnn_gsp_rows_backward_f32: beta * d loss / d out_feat stored straight into the buffer the last
+                     layer's input-gradient GEMM accumulates onto (zero-filled first when S < n), loss[0] += beta * loss
+
+    Every float equals the eager ``train_step(i, aux=lambda f: criterion_ppi.gpw_criterion(..., f, teacher_feat[i], kernel,
+    1, max_samples, sampled_inds=...)[2], beta)``.  The per-step buffers are sized for the largest graph and viewed at each
+    graph's own geometry, as gcrd.PerGraphGCRD's."""
+
+    NAME = "GSP"
+
+    def __init__(self, teacher_feat: Sequence[torch.Tensor], hidden: int, kernel: str = "rbf", beta: float = 100.0,
+                 max_samples: int = 8192, device="cuda"):
+        """teacher_feat: per training graph the teacher's [n_i, F_t] out_feat (``predict(..., return_feat=True)``; F_t = 1024
+        for TeacherNet); hidden: the student's out_feat width (136 for StudentNet), a multiple of 4 up to
+        lib.GSP_ROWS_MAX_F.  kernel 'cosine', 'poly', 'l2' or 'rbf' and max_samples 8192 are the argparse defaults of
+        ppi_pyg/gnn.py (8192 is above every PPI graph, so S = n).  The argparse beta default is 0, which switches the term
+        off, and scripts/run.sh has no gpw line; the PPI README tunes beta in {100, 1000, 10000}, so the default here is
+        100."""
+        if kernel not in criterion._KERNELS:
+            raise ValueError(f"kernel {kernel!r}: GSP kernels are {sorted(criterion._KERNELS)}")
+        if int(max_samples) < 1:
+            raise ValueError("max_samples must be at least 1")
+        if len(teacher_feat) == 0:
+            raise ValueError("no training graphs")
+        for k, t in enumerate(teacher_feat):
+            if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < 1:
+                raise ValueError(f"graph {k}: teacher features must be [n, F_t] with n, F_t >= 1")
+        widths = {int(t.shape[1]) for t in teacher_feat}
+        if len(widths) != 1:
+            raise ValueError(f"the teacher features have different widths {sorted(widths)}")
+        hidden = int(hidden)
+        if hidden % 4 or not 0 < hidden <= lib.GSP_ROWS_MAX_F:
+            raise ValueError(f"hidden width {hidden}: the GSP row passes take a multiple of 4 up to {lib.GSP_ROWS_MAX_F}")
+        self.device = dev = torch.device(device)
+        self.H, self.F_t, self.beta = hidden, widths.pop(), float(beta)
+        self.kernel, self.kernel_id = kernel, criterion._KERNELS[kernel]
+        sizes = [int(t.shape[0]) for t in teacher_feat]
+        samples = [min(int(max_samples), n) for n in sizes]
+
+        # the teacher similarities: one flat allocation, an [n, n] view per graph
+        offsets = [0]
+        for n in sizes:
+            offsets.append(offsets[-1] + n * n)
+        self.sim_flat = torch.empty(offsets[-1], dtype=torch.float32, device=dev)
+        self.sim_bytes = self.sim_flat.numel() * 4
+        sims = [self.sim_flat[o:o + n * n].view(n, n) for o, n in zip(offsets, sizes)]
+        for t, sim in zip(teacher_feat, sims):
+            self._build_sim(t.detach().to(dev, torch.float32).contiguous(), sim)
+
+        # the operands' padding rows must stay zero: every graph's S rows end at row S_max of one buffer, so the rows after
+        # them are written by no graph
+        H, S_max = self.H, max(samples)
+        flat_x = torch.zeros((S_max + 3) * H, device=dev)
+
+        def operands(S):
+            o = (S_max - S) * H
+            return flat_x[o:o + _ceil4(S) * H].view(_ceil4(S), H)
+
+        pool = _Pool(dev)
+        for n, S, sim in zip(sizes, samples, sims):
+            _GraphGSP(n, S, sim, operands(S), H, dev, pool.recorder())
+        self.graphs: List[_GraphGSP] = [_GraphGSP(n, S, sim, operands(S), H, dev, pool.views())
+                                        for n, S, sim in zip(sizes, samples, sims)]
+        self.loss_aux = self.graphs[0].loss_aux          # one float that every graph's view shares
+        n_draw = max((n for n, S in zip(sizes, samples) if S < n), default=0)
+        self.sample_ws = (torch.empty(int(lib.load().b200gnn_gcrd_sample_workspace_bytes(n_draw)), dtype=torch.uint8,
+                                      device=dev) if n_draw else None)
+        self._last = 0
+
+    def _build_sim(self, t: torch.Tensor, sim: torch.Tensor):
+        """sim [n, n] = the teacher similarities of all n rows of t, as gpw_criterion's chunk loop forms them with S = n."""
+        L, st = lib.load(), lib.stream_ptr()
+        n, k = t.shape[0], self.kernel_id
+        if k <= 1:
+            x, _ = criterion._normalize(t)
+            sq = None
+        else:
+            x, sq = t, torch.empty(n, dtype=torch.float32, device=t.device)
+            lib.check(L.b200gnn_row_sqnorm_f32(lib.dptr(x, torch.float32, "x"), n, x.shape[1], lib.dptr(sq, torch.float32, "sq"),
+                                               st), "row_sqnorm_f32")
+        x = criterion._pad_k(criterion._pad_k(x, 1), 0)                 # [Sp, F_t padded], as the eager operand
+        Sp = x.shape[0]
+        hi, lo = ops.split_tf32(x)
+        R = criterion.gsp_chunk_rows(Sp)
+        G = torch.empty(R, Sp, dtype=torch.float32, device=t.device)
+        for r0 in range(0, n, R):
+            r = min(R, n - r0)
+            ops.gemm_tf32x3(x[r0:r0 + r], hi, lo, out=G[:r])
+            lib.check(L.b200gnn_gsp_sim_chunk_f32(lib.dptr(G, torch.float32, "G"), Sp, r, n, r0,
+                                                  lib.dptr(sq, torch.float32, "sq"), k, lib.dptr(sim[r0], torch.float32, "sim"),
+                                                  n, st), "gsp_sim_chunk_f32")
+
+    def check_graphs(self, sizes: Sequence[int], hidden: int):
+        """ValueError unless the trainer's training graphs have these node counts and its out_feat this width (called by
+        PPIGATTrainer before any device work)."""
+        if len(sizes) != len(self.graphs):
+            raise ValueError(f"GSP built for {len(self.graphs)} training graphs, the trainer has {len(sizes)}")
+        if hidden != self.H:
+            raise ValueError(f"GSP built for hidden width {self.H}, the student's out_feat is {hidden} wide")
+        for k, (r, n) in enumerate(zip(self.graphs, sizes)):
+            if r.n != n:
+                raise ValueError(f"graph {k}: GSP built for {r.n} nodes, the trainer's graph has {n}")
+
+    def sample(self) -> torch.Tensor:
+        """The last step's sample: positions into the last graph's nodes (int64 [S])."""
+        return self.graphs[self._last].inds.to(torch.int64)
+
+    def check_sample(self, i: int, sample: torch.Tensor):
+        """ValueError unless ``sample`` is S_i distinct positions of graph i's nodes with S_i < n_i (PPIGATTrainer calls it
+        before the step launches anything)."""
+        r = self.graphs[i]
+        if r.S == r.n:
+            raise ValueError(f"GSP takes every row of graph {i} (max_samples >= {r.n}): there is no sample to inject")
+        s = torch.as_tensor(sample).to("cpu", torch.int64).view(-1)
+        if s.numel() != r.S or int(s.min()) < 0 or int(s.max()) >= r.n or s.unique().numel() != r.S:
+            raise ValueError(f"sample must hold {r.S} distinct positions in [0, {r.n})")
+
+    def forward_backward(self, i: int, tr, feat: torch.Tensor, d_feat: torch.Tensor, sample: Optional[torch.Tensor] = None):
+        """Graph i's objective: reads out_feat ``feat`` [n_i, H], writes d (beta * loss_aux) / d out_feat into d_feat
+        [n_i, H] (all rows; zero outside the sample), adds beta * loss_aux to tr.loss_out[0]; the value of loss_aux stays in
+        self.loss_aux.  Enqueues launches only (capturable) unless ``sample`` (positions into the graph's nodes, [S_i],
+        S_i < n_i) replaces the draw."""
+        r = self.graphs[i]
+        self._last = i
+        n, S, Sp, H, k = r.n, r.S, r.Sp, self.H, self.kernel_id
+        if sample is not None:
+            self.check_sample(i, sample)
+        draw_sample(tr, n, S, r.perm, self.sample_ws, sample)
+        L, st = lib.load(), lib.stream_ptr()
+        f = lambda t, name: lib.dptr(t, torch.float32, name)      # noqa: E731
+        inds = r.inds.data_ptr() if S < n else None
+        raw = k >= 2
+        lib.check(L.b200gnn_gsp_rows_operands_f32(f(feat, "feat"), feat.stride(0), inds, S, H, k, _EPS, f(r.x_s, "x_s"), H,
+                                                  f(r.norm, "norm"), st), "gsp_rows_operands_f32")
+        hi, lo = ops.split_tf32(r.x_s, hi=r.split[0], lo=r.split[1])
+        hiT, loT = ops.split_tf32(r.x_s, transpose=True, hi=r.splitT[0], lo=r.splitT[1])
+        R = r.G.shape[0]
+        for r0 in range(0, S, R):
+            m = min(R, S - r0)
+            ops.gemm_tf32x3(r.x_s[r0:r0 + m], hi, lo, out=r.G[:m])
+            lib.check(L.b200gnn_gsp_pair_fixed_chunk_f32(f(r.G, "G"), Sp, m, S, r0, f(r.norm if raw else None, "ns"),
+                                                         f(r.sim_t, "sim_t"), n, n, inds, k, f(r.rc if raw else None, "rc"),
+                                                         f(r.part, "part"), st), "gsp_pair_fixed_chunk_f32")
+            ops.gemm_tf32x3(r.G[:m], hiT, loT, out=r.g[r0:r0 + m])
+        lib.check(L.b200gnn_gsp_finish_f32(f(r.part, "part"), S, f(r.loss_aux, "loss"), st), "gsp_finish_f32")
+        if S < n:                  # rows outside the sample get no gradient; the buffer holds the previous step's
+            d_feat.zero_()
+        lib.check(L.b200gnn_gsp_rows_backward_f32(inds, S, H, k, f(r.g, "g"), f(r.x_s, "x_s"), H, f(r.norm, "norm"),
+                                                  f(r.rc, "rc"), _EPS, self.beta, f(d_feat, "d_feat"), d_feat.stride(0),
+                                                  f(r.loss_aux, "loss_aux"), f(tr.loss_out, "loss_out"), st),
+                  "gsp_rows_backward_f32")

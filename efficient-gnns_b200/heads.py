@@ -96,6 +96,23 @@ class HeadRows:
         heads._objective_buffers(self, alloc)
 
 
+def draw_sample(tr, n: int, S: int, perm: torch.Tensor, workspace: Optional[torch.Tensor], sample: Optional[torch.Tensor]):
+    """The step's sample of S of n rows into perm[:S] (int32 [n]): the injected ``sample``, or, when S < n, the on-device
+    draw at (trainer seed, SAMPLE_STREAM, the trainer's device step counter) on ``workspace``
+    (b200gnn_gcrd_sample_workspace_bytes(n) bytes).  Nothing when S = n and no sample is given."""
+    if sample is not None:
+        # the kernels index rows and store gradient rows by these positions: refuse what would go out of bounds or store
+        # one row twice (the override runs eagerly, so a host check costs nothing the step depends on)
+        s = torch.as_tensor(sample).to("cpu", torch.int64).view(-1)
+        if s.numel() != S or (S and (int(s.min()) < 0 or int(s.max()) >= n)) or s.unique().numel() != S:
+            raise ValueError(f"sample must hold {S} distinct positions in [0, {n})")
+        perm[:S].copy_(s.to(torch.int32))
+    elif S < n:
+        L = lib.load()
+        lib.check(L.b200gnn_gcrd_sample_i32(n, tr.seed, SAMPLE_STREAM, lib.dptr(tr.step_count, torch.int32, "step"),
+                                            perm.data_ptr(), workspace.data_ptr(), lib.stream_ptr()), "gcrd_sample_i32")
+
+
 def check_widths(hidden: int, proj_dim: int, teacher_width: int):
     """ValueError for a head shape the step's kernels do not take."""
     if not ops.gemm_stats_supported(proj_dim):
@@ -258,19 +275,7 @@ class ProjectionHeads:
 
     def _draw(self, tr, r: HeadRows, sample: Optional[torch.Tensor]):
         """The step's sample into r.perm: the injected one, or the on-device draw when S < n (none when S = n)."""
-        n, S = r.n, r.S
-        if sample is not None:
-            # the kernels index pre_s / pre_t and store dz rows by these positions: refuse what would go out of bounds or
-            # store one row twice (the override runs eagerly, so a host check costs nothing the step depends on)
-            s = torch.as_tensor(sample).to("cpu", torch.int64).view(-1)
-            if s.numel() != S or (S and (int(s.min()) < 0 or int(s.max()) >= n)) or s.unique().numel() != S:
-                raise ValueError(f"sample must hold {S} distinct positions in [0, {n})")
-            r.perm[:S].copy_(s.to(torch.int32))
-        elif S < n:
-            L = lib.load()
-            lib.check(L.b200gnn_gcrd_sample_i32(n, tr.seed, SAMPLE_STREAM, lib.dptr(tr.step_count, torch.int32, "step"),
-                                                r.perm.data_ptr(), self.sample_ws.data_ptr(), lib.stream_ptr()),
-                      "gcrd_sample_i32")
+        draw_sample(tr, r.n, r.S, r.perm, self.sample_ws, sample)
 
     def _front(self, r: HeadRows, G_s: torch.Tensor):
         """Both heads' Linear over the row set with the BatchNorm statistics in the GEMM epilogue, then finalize (running

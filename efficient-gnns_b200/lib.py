@@ -18,6 +18,7 @@ OK = 0
 REDUCE_SUM = 0
 REDUCE_MEAN = 1
 LSP_MAX_F = 512          # B200GNN_LSP_MAX_F: widest student row b200gnn_lsp_student_f32 holds in registers
+GSP_ROWS_MAX_F = 2048    # B200GNN_GSP_ROWS_MAX_F: widest feature row of the fixed-teacher GSP row passes
 
 _i32p = C.c_void_p
 _f32p = C.c_void_p
@@ -142,6 +143,12 @@ SIGNATURES = {
     "b200gnn_gsp_backward_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32,
                                         _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_row_axpy_f32": (_int, [_f32p, _f32p, _i64, _i64, _f32, _f32p, _ptr]),
+    "b200gnn_gsp_sim_chunk_f32": (_int, [_f32p, _i64, _i64, _i64, _i64, _f32p, _int, _f32p, _i64, _ptr]),
+    "b200gnn_gsp_pair_fixed_chunk_f32": (_int, [_f32p, _i64, _i64, _i64, _i64, _f32p, _f32p, _i64, _i64, _i32p, _int, _f32p,
+                                                _f32p, _ptr]),
+    "b200gnn_gsp_rows_operands_f32": (_int, [_f32p, _i64, _i32p, _i64, _i64, _int, _f32, _f32p, _i64, _f32p, _ptr]),
+    "b200gnn_gsp_rows_backward_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _i64, _f32p, _f32p, _f32, _f32, _f32p, _i64,
+                                             _f32p, _f32p, _ptr]),
     "b200gnn_edge_sim_f32": (_int, [_f32p, _i64, _i32p, _i32p, _i64, _int, _f32p, _ptr]),
     "b200gnn_lsp_partials": (_i64, [_i64]),
     "b200gnn_lsp_segment_f32": (_int, [_f32p, _f32p, _i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _ptr]),

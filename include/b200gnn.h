@@ -543,6 +543,32 @@ int b200gnn_gsp_backward_f32(const int32_t* inds, int64_t S, int64_t P, int kern
                              const float* rc_t, float eps, const float* pre_s, const float* bn_s, const float* pre_t,
                              const float* bn_t, float beta, float* dz_s, float* dz_t, float* part_s, float* part_t,
                              const float* loss_aux, float* loss_total, void* stream);
+/* GSP against a fixed teacher (csrc/loss_pair.cu; the PPI step, gpw_criterion on model.out_feat and the frozen teacher's
+ * out_feat, ppi_pyg/gnn.py:230-239): the teacher's n x n similarity matrix is built once, the step runs the student side.
+ *   gsp_sim_chunk: sim = rows [row_offset, row_offset + n_rows) of the similarity matrix from the same rows of the Gram
+ *     matrix (G pitch ldg >= n, sim pitch ld_sim >= n, both at the chunk's first row); kernels 2,3 need sq[n], the squared
+ *     row norms; the l2 / rbf diagonal is exactly 0.  Each entry equals the teacher similarity b200gnn_gsp_pair_chunk_f32
+ *     forms from the same Gram entry.
+ *   gsp_pair_fixed_chunk: the student side of b200gnn_gsp_pair_chunk_f32 (Gs, ld, rows, ns, rc_s, partial: the same
+ *     meaning and bits) with sim_t read from the stored [n_t, n_t] matrix (pitch ld_t) at [inds[i]][inds[j]]; inds[S]
+ *     nullable (the identity, S <= n_t); the l2 / rbf diagonal is the sample position.
+ *   gsp_rows_operands: x[j] (pitch ldx) = feat[inds[j]] (pitch ldf; inds nullable: row j) normalised with eps, norm[j] its
+ *     norm (kernels 0,1: row_normalize_fwd's arithmetic), or copied, norm[j] its squared norm (kernels 2,3: row_sqnorm's).
+ *   gsp_rows_backward: d_feat[inds[j]] (pitch ldd) = beta * d, d = normalise backward of 2 g[j] (kernels 0,1; norm
+ *     required) or 2 g[j] + 4 rc[j] x[j] (kernels 2,3; rc required), g = dG . x; the arithmetic of row_normalize_bwd /
+ *     row_axpy, then the multiply by beta.  loss_total[0] += beta * loss_aux[0] (two roundings) when loss_total is given.
+ * F (the feature width) is at most B200GNN_GSP_ROWS_MAX_F, the widest layer the PPI engine stores. */
+#define B200GNN_GSP_ROWS_MAX_F 2048
+int b200gnn_gsp_sim_chunk_f32(const float* G, int64_t ldg, int64_t n_rows, int64_t n, int64_t row_offset, const float* sq,
+                              int kernel, float* sim, int64_t ld_sim, void* stream);
+int b200gnn_gsp_pair_fixed_chunk_f32(float* Gs, int64_t ld, int64_t n_rows, int64_t S, int64_t row_offset, const float* ns,
+                                     const float* sim_t, int64_t ld_t, int64_t n_t, const int32_t* inds, int kernel,
+                                     float* rc_s, float* partial, void* stream);
+int b200gnn_gsp_rows_operands_f32(const float* feat, int64_t ldf, const int32_t* inds, int64_t S, int64_t F, int kernel,
+                                  float eps, float* x, int64_t ldx, float* norm, void* stream);
+int b200gnn_gsp_rows_backward_f32(const int32_t* inds, int64_t S, int64_t F, int kernel, const float* g, const float* x,
+                                  int64_t ldx, const float* norm, const float* rc, float eps, float beta, float* d_feat,
+                                  int64_t ldd, const float* loss_aux, float* loss_total, void* stream);
 /* y[i,:] += alpha * coef[i] * x[i,:] */
 int b200gnn_row_axpy_f32(const float* x, const float* coef, int64_t n, int64_t F,
                          float alpha, float* y, void* stream);
