@@ -10,6 +10,11 @@
 //   saint_subgraph  induced subgraph of a SORTED UNIQUE node set S over CSR: a node -> local-id map, one warp per selected
 //                   row counting / writing the edges whose column is in S (ballot prefix: CSR order preserved, as
 //                   SparseTensor.saint_subgraph keeps it), with the edge ids of the parent graph for attribute slicing.
+//   induced_edges   the edges of a batch whose endpoints are both marked in a node mask, relabelled to the endpoints'
+//                   ranks among the marked nodes, edge order kept (torch_geometric.utils.subgraph(mask.nonzero(), edge_index,
+//                   relabel_nodes=True)[0], the LSP edge list of mag_pyg/gnn_kd_and_aux.py:240-243).  One block scans the
+//                   mask into ranks; tiles of IE_TILE edges count their kept edges, one block scans the tile counts, and
+//                   the fill rescans each tile with a block prefix sum, so every kept edge lands at its rank in edge order.
 // Integer / index work: bit-exact against oracle/sampling.py.
 #include "common.cuh"
 #include "philox.cuh"
@@ -71,6 +76,140 @@ __global__ void __launch_bounds__(256) induced_rows_kernel(const int32_t* __rest
   if (!FILL && lane == 0) counts_or_ptr[i] = cnt;
 }
 
+// ---- induced_edges
+constexpr int IE_THREADS = 256, IE_ITEMS = 4, IE_TILE = IE_THREADS * IE_ITEMS;
+constexpr int SCAN_THREADS = 1024;
+
+// Exclusive prefix sum over the block (blockDim.x == NT); returns the thread's exclusive prefix, *total gets the block sum.
+template <int NT>
+__device__ __forceinline__ int64_t block_exclusive_scan(int64_t v, int64_t* total) {
+  __shared__ int64_t warp_sum[NT / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int64_t inc = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int64_t o = __shfl_up_sync(FULL_MASK, inc, d);
+    if (lane >= d) inc += o;
+  }
+  if (lane == 31) warp_sum[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    int64_t w = lane < NT / 32 ? warp_sum[lane] : 0;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int64_t o = __shfl_up_sync(FULL_MASK, w, d);
+      if (lane >= d) w += o;
+    }
+    if (lane < NT / 32) warp_sum[lane] = w;                  // inclusive over warps
+  }
+  __syncthreads();
+  const int64_t before = warp == 0 ? 0 : warp_sum[warp - 1];
+  *total = warp_sum[NT / 32 - 1];
+  return before + inc - v;
+}
+
+// One block: out[i] = sum_{j<i} load(j) over [0, n) in contiguous per-thread chunks (exclusive scan); total[0] = the sum.
+template <typename Load>
+__device__ __forceinline__ void single_block_scan(Load load, int64_t n, int64_t* __restrict__ out, int64_t* __restrict__ total) {
+  const int64_t chunk = (n + SCAN_THREADS - 1) / SCAN_THREADS;
+  const int64_t b = min(n, (int64_t)threadIdx.x * chunk), e = min(n, b + chunk);
+  int64_t s = 0;
+  for (int64_t i = b; i < e; ++i) s += load(i);
+  int64_t all;
+  int64_t run = block_exclusive_scan<SCAN_THREADS>(s, &all);
+  for (int64_t i = b; i < e; ++i) {
+    const int64_t v = load(i);
+    out[i] = run;
+    run += v;
+  }
+  if (threadIdx.x == 0) *total = all;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) mask_rank_kernel(const uint8_t* __restrict__ mask, int64_t n,
+                                                                 int64_t* __restrict__ rank, int64_t* __restrict__ n_marked) {
+  single_block_scan([&](int64_t i) -> int64_t { return mask[i] != 0; }, n, rank, n_marked);
+}
+
+// Kept / out-of-range flags of the IE_ITEMS consecutive edges of this thread (bit k: edge tile·IE_TILE + t·IE_ITEMS + k).
+__device__ __forceinline__ void induced_flags(const int64_t* __restrict__ ei, int64_t ld, int64_t E, const uint8_t* __restrict__ mask,
+                                              int64_t n, int64_t first, unsigned& keep, int& bad) {
+  keep = 0u;
+  bad = 0;
+#pragma unroll
+  for (int k = 0; k < IE_ITEMS; ++k) {
+    const int64_t j = first + k;
+    if (j >= E) break;
+    const int64_t s = ei[j], d = ei[ld + j];
+    if (s < 0 || s >= n || d < 0 || d >= n) {
+      ++bad;
+      continue;
+    }
+    if (mask[s] && mask[d]) keep |= 1u << k;
+  }
+}
+
+__global__ void __launch_bounds__(IE_THREADS) induced_count_kernel(const int64_t* __restrict__ ei, int64_t ld, int64_t E,
+                                                                   const uint8_t* __restrict__ mask, int64_t n, int64_t n_tiles,
+                                                                   int64_t* __restrict__ tile_cnt) {
+  unsigned keep;
+  int bad;
+  induced_flags(ei, ld, E, mask, n, (int64_t)blockIdx.x * IE_TILE + threadIdx.x * IE_ITEMS, keep, bad);
+  int64_t all_kept, all_bad;
+  block_exclusive_scan<IE_THREADS>(__popc(keep), &all_kept);
+  __syncthreads();                                           // warp_sum is reused by the second scan
+  block_exclusive_scan<IE_THREADS>(bad, &all_bad);
+  if (threadIdx.x == 0) {
+    tile_cnt[blockIdx.x] = all_kept;
+    tile_cnt[n_tiles + blockIdx.x] = all_bad;
+  }
+}
+
+// tile_cnt [2, n_tiles] (kept, out of range) -> tile_cnt[0] := exclusive offsets of the kept edges; totals = {kept, bad}.
+__global__ void __launch_bounds__(SCAN_THREADS) induced_scan_kernel(int64_t* __restrict__ tile_cnt, int64_t n_tiles,
+                                                                    int64_t* __restrict__ totals) {
+  int64_t s = 0;
+  for (int64_t i = threadIdx.x; i < n_tiles; i += SCAN_THREADS) s += tile_cnt[n_tiles + i];
+  int64_t bad;
+  block_exclusive_scan<SCAN_THREADS>(s, &bad);
+  __syncthreads();
+  // the in-place scan reads each count before any thread overwrites it: every thread owns one contiguous chunk
+  const int64_t chunk = (n_tiles + SCAN_THREADS - 1) / SCAN_THREADS;
+  const int64_t b = min(n_tiles, (int64_t)threadIdx.x * chunk), e = min(n_tiles, b + chunk);
+  int64_t c = 0;
+  for (int64_t i = b; i < e; ++i) c += tile_cnt[i];
+  int64_t kept;
+  int64_t run = block_exclusive_scan<SCAN_THREADS>(c, &kept);
+  for (int64_t i = b; i < e; ++i) {
+    const int64_t v = tile_cnt[i];
+    tile_cnt[i] = run;
+    run += v;
+  }
+  if (threadIdx.x == 0) {
+    totals[0] = kept;
+    totals[1] = bad;
+  }
+}
+
+__global__ void __launch_bounds__(IE_THREADS) induced_fill_kernel(const int64_t* __restrict__ ei, int64_t ld, int64_t E,
+                                                                  const uint8_t* __restrict__ mask, int64_t n,
+                                                                  const int64_t* __restrict__ rank, const int64_t* __restrict__ tile_off,
+                                                                  int64_t* __restrict__ out, int64_t ld_out) {
+  const int64_t first = (int64_t)blockIdx.x * IE_TILE + threadIdx.x * IE_ITEMS;
+  unsigned keep;
+  int bad;
+  induced_flags(ei, ld, E, mask, n, first, keep, bad);
+  int64_t all;
+  int64_t o = tile_off[blockIdx.x] + block_exclusive_scan<IE_THREADS>(__popc(keep), &all);
+#pragma unroll
+  for (int k = 0; k < IE_ITEMS; ++k) {
+    if (keep & (1u << k)) {
+      out[o] = rank[ei[first + k]];
+      out[ld_out + o] = rank[ei[ld + first + k]];
+      ++o;
+    }
+  }
+}
+
 }  // namespace sampling
 }  // namespace b200gnn
 
@@ -111,5 +250,48 @@ extern "C" int b200gnn_saint_subgraph_fill_i64(const int32_t* rowptr, const int3
   if (n_sel == 0) return B200GNN_OK;
   sampling::induced_rows_kernel<true><<<(unsigned)((n_sel * 32 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       rowptr, col, eid, nodes, n_sel, node_map, const_cast<int64_t*>(out_ptr), out_row, out_col, out_eid);
+  return check_launch();
+}
+
+extern "C" int64_t b200gnn_induced_edges_tiles(int64_t n_edges) {
+  return n_edges < 0 ? -1 : (n_edges + sampling::IE_TILE - 1) / sampling::IE_TILE;
+}
+
+// edge_index: int64 rows src (edge_index[0..E)) and dst (edge_index[ld..ld+E)); mask: uint8 / bool [n_nodes].
+// rank: int64 [n_nodes + 1] workspace, on return the number of marked nodes before each node (rank[n_nodes]: all); tile_cnt: int64
+// [2 * b200gnn_induced_edges_tiles(E)] workspace; totals: int64 [2] = {kept edges, edges with an endpoint outside [0, n)}.
+extern "C" int b200gnn_induced_edges_count_i64(const int64_t* edge_index, int64_t ld, int64_t n_edges, const uint8_t* mask,
+                                               int64_t n_nodes, int64_t* rank, int64_t* tile_cnt, int64_t* totals, void* stream) {
+  if (!mask || !rank || !totals || n_nodes < 0 || n_edges < 0 || (n_edges > 0 && (!edge_index || !tile_cnt || ld < n_edges)))
+    return B200GNN_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  sampling::mask_rank_kernel<<<1, sampling::SCAN_THREADS, 0, st>>>(mask, n_nodes, rank, rank + n_nodes);
+  int rc;
+  if ((rc = check_launch())) return rc;
+  const int64_t tiles = b200gnn_induced_edges_tiles(n_edges);
+  if (tiles == 0) {
+    if (cudaMemsetAsync(totals, 0, 2 * sizeof(int64_t), st) != cudaSuccess) return B200GNN_ERR_CUDA;
+    return B200GNN_OK;
+  }
+  if (tiles > 0x7fffffffLL) return B200GNN_ERR_BAD_ARG;
+  sampling::induced_count_kernel<<<(unsigned)tiles, sampling::IE_THREADS, 0, st>>>(edge_index, ld, n_edges, mask, n_nodes, tiles,
+                                                                                  tile_cnt);
+  if ((rc = check_launch())) return rc;
+  sampling::induced_scan_kernel<<<1, sampling::SCAN_THREADS, 0, st>>>(tile_cnt, tiles, totals);
+  return check_launch();
+}
+
+// tile_cnt: as the count call left it; out: int64 rows (out[0..kept) relabelled sources, out[ld_out..ld_out+kept) destinations).
+extern "C" int b200gnn_induced_edges_fill_i64(const int64_t* edge_index, int64_t ld, int64_t n_edges, const uint8_t* mask,
+                                              int64_t n_nodes, const int64_t* rank, const int64_t* tile_cnt, int64_t* out,
+                                              int64_t ld_out, void* stream) {
+  if (!mask || !rank || n_nodes < 0 || n_edges < 0 || ld_out < 0 ||
+      (n_edges > 0 && (!edge_index || !tile_cnt || !out || ld < n_edges)))
+    return B200GNN_ERR_BAD_ARG;
+  const int64_t tiles = b200gnn_induced_edges_tiles(n_edges);
+  if (tiles == 0) return B200GNN_OK;
+  if (tiles > 0x7fffffffLL) return B200GNN_ERR_BAD_ARG;
+  sampling::induced_fill_kernel<<<(unsigned)tiles, sampling::IE_THREADS, 0, (cudaStream_t)stream>>>(
+      edge_index, ld, n_edges, mask, n_nodes, rank, tile_cnt, out, ld_out);
   return check_launch();
 }

@@ -88,6 +88,9 @@ SIGNATURES = {
     "b200gnn_random_walk_i64": (_int, [_i32p, _i32p, _i64, _ptr, _i64, _i32, _u64, _u64, _ptr, _ptr]),
     "b200gnn_saint_subgraph_count_i64": (_int, [_i32p, _i32p, _ptr, _i64, _i32p, _ptr, _ptr]),
     "b200gnn_saint_subgraph_fill_i64": (_int, [_i32p, _i32p, _ptr, _ptr, _i64, _i32p, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "b200gnn_induced_edges_tiles": (_i64, [_i64]),
+    "b200gnn_induced_edges_count_i64": (_int, [_ptr, _i64, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _ptr]),
+    "b200gnn_induced_edges_fill_i64": (_int, [_ptr, _i64, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _i64, _ptr]),
     "b200gnn_gemm_stat_slots": (_i64, [_i64, _i64]),
     "b200gnn_gemm_set_bnbwd_variant": (None, [_int]),
     "b200gnn_gemm_tf32x3_stats_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p, _int, _f32p, _i64,

@@ -25,6 +25,10 @@ beta=beta)``: the same kernels' arithmetic, the same SpMM, and beta applied as i
 
 ``PerGraphLSP`` is the same loss for engine_ppi's PPI student: one raw edge list per training graph, every node a row, the
 constants of each graph built once by the helpers ``LSP`` uses and the step's buffers shared by all graphs.
+
+``BatchLSP`` is the same loss for rgcn's MAG student on GraphSAINT batches, where nothing is a constant of the run: each
+batch has its own train-induced edge list (built on the device, sampling.induced_edges) and the teacher runs inside the
+student's step, so the plan, the backward matrix and sim_t are built per batch by the same helpers.
 """
 from __future__ import annotations
 
@@ -32,7 +36,7 @@ from typing import Optional, Sequence
 
 import torch
 
-from . import criterion, lib, ops
+from . import criterion, lib, ops, sampling
 
 _KERNELS = criterion._KERNELS             # PerGraphLSP's criterion= argument shadows the module
 
@@ -207,3 +211,79 @@ class PerGraphLSP:
                         self.sim_s[:E], self.scratch[:2 * E], g.C.val, g.selfc, self.loss_aux, self.partial)
         d = ops.spmm_csr(g.C, feat, "sum", out=self.d[:n])
         ops.scatter_rows_scaled(d, self.rows[:n], self.beta, d_feat, loss_aux=self.loss_aux, loss_total=loss_out)
+
+
+class BatchLSP:
+    """LSP inside rgcn.RGCNTrainer's step: the reference's MAG ``train()`` with ``--training lpw``
+    (mag_pyg/gnn_kd_and_aux.py:232-245) on every GraphSAINT batch b:
+
+        edge_index = subgraph(b.train_mask.nonzero().squeeze(1), b.edge_index, relabel_nodes=True)[0]
+        loss_aux   = lpw_criterion(out, labels, model.out_feat[b.train_mask], teacher_model.out_feat[b.train_mask],
+                                   edge_index, kernel, beta)[2]                    kld
+        loss       = kd_criterion(out, labels, teacher_out, alpha, kd_T)[0] + beta * loss_aux
+
+    Per batch, between the student's loss and its backward (``RGCNTrainer(..., lsp=o).train_step(b, x, teacher=t)``):
+
+        edges      sampling.induced_edges (one host read sizes it), then the dst-sorted plan, the backward matrix for
+                   n_train rows and the teacher's sim_t (_edge_constants, as LSP builds them once)
+        gather     G_s = the student's last hidden layer (after ReLU and dropout) and G_t = the teacher's (eval: ReLU) at
+                   the train rows, in the order of train_mask.nonzero()
+        student    b200gnn_lsp_student_f32, then d = C . G_s (the row-segmented SpMM)
+        backward   beta * d scattered straight into the internal-order gradient the trainer adds at its last hidden layer,
+                   loss[0] += beta * loss_aux (b200gnn_scatter_rows_scaled_f32); loss[2] = loss_aux
+
+    The train rows are relabelled by their rank in train_mask.nonzero() (batch order) and gathered at their internal rows
+    BatchPlan.pos[train_mask.nonzero()], so row k of G_s is the k-th train row whatever the internal order.  (All train
+    rows are papers and BatchPlan sorts types stably, so those internal rows also ascend.)
+
+    Every float equals the eager ``train_step(b, x, teacher_logits=..., aux=lambda f: criterion.lpw_criterion(...,
+    f[train_mask], t_feat[train_mask], edge_index, kernel, 1)[2], beta=beta)``.  A batch whose train rows induce no edge
+    does what the reference does: kl_div's mean over no term is NaN, so loss[0] and loss[2] are NaN, and the step's
+    gradients carry no LSP term."""
+
+    def __init__(self, hidden: int, kernel: str = "rbf", beta: float = 1.0, criterion: str = "kld", device="cuda"):
+        """hidden: the student's last hidden width (32 in the reference's MAG student), at most lib.LSP_MAX_F.  kernel:
+        'cosine', 'poly', 'l2' or 'rbf' (scripts/run_kd_and_aux.sh runs rbf, cosine and poly); beta: the weight of the loss.
+        Only the kld criterion (the reference's default) is built."""
+        if kernel not in _KERNELS:
+            raise ValueError(f"kernel {kernel!r}: LSP kernels are {sorted(_KERNELS)}")
+        if criterion != "kld":
+            raise ValueError(f"criterion {criterion!r}: the fused LSP step is the kld form (the reference's default)")
+        if not 0 < int(hidden) <= lib.LSP_MAX_F:
+            raise ValueError(f"hidden width {hidden}: the LSP kernel holds a student row in registers, at most {lib.LSP_MAX_F}")
+        self.device = torch.device(device)
+        self.H, self.kernel, self.kernel_id, self.beta = int(hidden), kernel, _KERNELS[kernel], float(beta)
+        self.loss_aux = torch.zeros(1, dtype=torch.float32, device=self.device)
+        self.edge_index: Optional[torch.Tensor] = None          # the last batch's train-induced edge list
+
+    def bind(self, trainer):
+        """Called by the RGCNTrainer that owns this object: its last hidden layer must be the width built for."""
+        if trainer.L < 2 or trainer.dims[-2] != self.H:
+            raise ValueError(f"LSP built for hidden width {self.H}, the student's last hidden layer is "
+                             f"{trainer.dims[-2] if trainer.L >= 2 else 'absent'}")
+
+    def forward_backward(self, tr, teacher, batch) -> Optional[torch.Tensor]:
+        """After tr's loss on its forward and teacher's eval forward on the same plan: returns d (beta * loss_aux) / d out_feat
+        [N, H] in internal row order (None when the batch induces no edge) and adds beta * loss_aux to tr.loss_out[0]."""
+        f, ft = tr._fwd, teacher._fwd
+        P, train_int = f["P"], f["train_int"]
+        n = train_int.numel()
+        ei = sampling.induced_edges(batch.edge_index, batch.train_mask.view(-1))
+        self.edge_index = ei
+        if ei.shape[1] == 0:
+            self.loss_aux.fill_(float("nan"))
+            tr.loss_out[:1].add_(self.loss_aux * self.beta)
+            return None
+        feat_t = ft["xs"][-1]
+        G_t = ops.gather_rows_act(feat_t, train_int, torch.empty(n, feat_t.shape[1], device=self.device))
+        plan, (C, pos_dst, pos_src, diag_pos, selfc), sim_t = _edge_constants(G_t, ei, n, self.kernel_id)
+        del G_t
+        G_s = ops.gather_rows_act(f["xs"][-1], train_int, torch.empty(n, self.H, device=self.device))
+        E = plan.E
+        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=self.device)    # noqa: E731
+        ops.lsp_student(G_s, plan.src, plan.dst, plan.rowptr, sim_t, self.kernel_id, pos_dst, pos_src, C.rowptr, diag_pos,
+                        e(E), e(2 * E), C.val, selfc, self.loss_aux, e(int(lib.load().b200gnn_lsp_partials(plan.n_seg))))
+        d = ops.spmm_csr(C, G_s, "sum")
+        d_feat = torch.zeros(P.N, self.H, device=self.device)
+        ops.scatter_rows_scaled(d, train_int, self.beta, d_feat, loss_aux=self.loss_aux, loss_total=tr.loss_out)
+        return d_feat

@@ -266,7 +266,8 @@ class RGCNTrainer:
 
     def __init__(self, in_channels: int, hidden_channels: int, out_channels: int, num_layers: int, dropout: float,
                  num_nodes_dict: Dict[int, int], x_types, num_edge_types: int, relations: Dict[int, Tuple[int, int]],
-                 lr: float = 0.01, seed: int = 0, alpha: float = 0.9, kd_T: float = 4.0, device="cuda"):
+                 lr: float = 0.01, seed: int = 0, alpha: float = 0.9, kd_T: float = 4.0, device="cuda", lsp=None):
+        """lsp: an lsp.BatchLSP run inside every step (the reference's ``--training lpw``); its steps take ``teacher=``."""
         self.dev = torch.device(device)
         self.F_in, self.H, self.C, self.L = int(in_channels), int(hidden_channels), int(out_channels), int(num_layers)
         self.p, self.lr, self.alpha, self.kd_T, self.seed = float(dropout), float(lr), float(alpha), float(kd_T), int(seed)
@@ -278,6 +279,7 @@ class RGCNTrainer:
         self.R = int(num_edge_types)
         if sorted(int(r) for r in relations) != list(range(self.R)):
             raise lib.B200GnnError("relations must map every edge type 0..R-1 to its (source type, destination type)")
+        self.relations = tuple((int(relations[r][0]), int(relations[r][1])) for r in range(self.R))
         self.rel_src = torch.tensor([int(relations[r][0]) for r in range(self.R)], dtype=torch.long, device=self.dev)
         self.rel_dst = torch.tensor([int(relations[r][1]) for r in range(self.R)], dtype=torch.long, device=self.dev)
         self.rels_of = [[r for r in range(self.R) if int(relations[r][1]) == t] for t in range(self.T)]
@@ -307,6 +309,9 @@ class RGCNTrainer:
         self.reset_parameters(seed)
         self._fwd = None
         self._training = False
+        self.lsp = lsp
+        if lsp is not None:
+            lsp.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def _wcatT(self, i: int, t: int, buf: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -381,10 +386,12 @@ class RGCNTrainer:
         return BatchPlan(batch.edge_index, batch.edge_attr, batch.node_type, self.rel_src, self.rel_dst, self.T)
 
     # ------------------------------------------------------------------ forward / backward
-    def forward(self, batch, x_dict: Dict[int, torch.Tensor], training: bool = True) -> torch.Tensor:
-        """Logits [n_batch, C] in the batch's node order; ``training=False``: no dropout (the teacher's eval forward)."""
+    def forward(self, batch, x_dict: Dict[int, torch.Tensor], training: bool = True,
+                plan: Optional[BatchPlan] = None) -> torch.Tensor:
+        """Logits [n_batch, C] in the batch's node order; ``training=False``: no dropout (the teacher's eval forward).
+        ``plan``: the batch's BatchPlan when the caller already has it (a teacher running on its student's plan)."""
         self._training = bool(training)
-        P = self.plan(batch)
+        P = self.plan(batch) if plan is None else plan
         G, Gt = P.graphs()
         li_int = batch.local_node_idx.view(-1).long()[P.perm].contiguous()
         tables = {int(t): v for t, v in x_dict.items()}
@@ -420,9 +427,11 @@ class RGCNTrainer:
         f = self._fwd
         return f["xs"][-1][f["P"].pos]
 
-    def backward(self, d_logits_int: torch.Tensor, d_out_feat: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def backward(self, d_logits_int: torch.Tensor, d_out_feat: Optional[torch.Tensor] = None,
+                 d_out_feat_int: Optional[torch.Tensor] = None) -> torch.Tensor:
         """d loss / d logits [N, C'] in INTERNAL row order -> self.grads (flat) and the returned layer-0 input gradient [N, F_in]
-        (internal order).  d_out_feat (batch order) is added to the gradient arriving at the last hidden activation."""
+        (internal order).  d_out_feat (batch order) or d_out_feat_int (internal order) is added to the gradient arriving at
+        the last hidden activation."""
         f = self._fwd
         P = f["P"]
         self.grads.zero_()
@@ -450,17 +459,21 @@ class RGCNTrainer:
             if i > 0:
                 if i == self.L - 1 and d_out_feat is not None:
                     dx.add_(d_out_feat[P.perm])
+                if i == self.L - 1 and d_out_feat_int is not None:
+                    dx.add_(d_out_feat_int)
                 dy = ops.relu_dropout_bwd(dx, f["xs"][i], self.p if self._training else 0.0, out=dx)
         return dx
 
-    def _loss(self, P, batch, teacher_logits) -> torch.Tensor:
-        """Fused CE / KD over the train_mask rows on the padded logits (ld = C'); returns d logits (internal order)."""
+    def _loss(self, P, batch, teacher_logits, teacher_int: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Fused CE / KD over the train_mask rows on the padded logits (ld = C'); returns d logits (internal order).
+        teacher_int: the teacher's padded logits in internal row order, read in place (a teacher run on this plan)."""
         y_int = batch.y.view(-1).long()[P.perm].contiguous()
         train_b = batch.train_mask.view(-1).nonzero().view(-1)
         train_int = P.pos[train_b].contiguous()
+        self._fwd["train_int"] = train_int
         logits = self._fwd["ys"][-1]
         d = torch.zeros_like(logits)
-        teacher = None
+        teacher = teacher_int
         if teacher_logits is not None:
             teacher = torch.zeros(P.N, self.C, device=self.dev)
             teacher[train_int] = teacher_logits.to(torch.float32)
@@ -474,19 +487,51 @@ class RGCNTrainer:
             "kd_loss_fwd_bwd_f32")
         return d
 
+    def check_teacher(self, teacher: "RGCNTrainer") -> None:
+        """ValueError unless ``teacher`` can run on this trainer's batch plans and feed its loss: the same node types and
+        table sizes, feature types, relations (source, destination), input width, classes and device."""
+        if not isinstance(teacher, RGCNTrainer):
+            raise ValueError("teacher= must be an RGCNTrainer")
+        for what, mine, theirs in (("node types and counts", self.num_nodes, teacher.num_nodes),
+                                   ("node types with features", self.x_types, teacher.x_types),
+                                   ("relations (source type, destination type)", self.relations, teacher.relations),
+                                   ("input width", self.F_in, teacher.F_in), ("classes", self.C, teacher.C),
+                                   ("device", self.dev, teacher.dev)):
+            if mine != theirs:
+                raise ValueError(f"teacher= has other {what} than the student ({theirs} vs {mine}): it cannot run on the "
+                                 "student's batch plan")
+
     def train_step(self, batch, x_dict: Dict[int, torch.Tensor], teacher_logits: Optional[torch.Tensor] = None, aux=None,
-                   beta: float = 1.0) -> torch.Tensor:
+                   beta: float = 1.0, teacher: Optional["RGCNTrainer"] = None) -> torch.Tensor:
         """One iteration of the reference ``train()`` loop body: logit-KD if ``teacher_logits`` ([n_train, C], the teacher's
-        logits on the train_mask rows in batch order) is given, else cross-entropy, over the train_mask rows; then Adam over
-        every parameter and embedding row.  ``aux(out_feat)`` as in ``GCNStudentTrainer.train_step``.  Returns the device
-        tensor [loss, loss_cls, loss_kd]."""
+        logits on the train_mask rows in batch order) or ``teacher`` is given, else cross-entropy, over the train_mask rows;
+        then Adam over every parameter and embedding row.  ``aux(out_feat)`` as in ``GCNStudentTrainer.train_step``.
+
+        ``teacher``: another RGCNTrainer (the reference's ``teacher_model``), run in eval mode on this step's batch plan (one
+        plan per batch, no second sort); the KD loss reads its padded logits in place, and nothing of the teacher changes.
+        The trainer's ``lsp=`` objective needs it: the teacher's last hidden layer (ReLU, no dropout) is its feature side.
+        Returns the device tensor [loss, loss_cls, loss_kd] ([kd + beta * lsp, loss_cls, lsp] with lsp=)."""
+        if teacher is not None and teacher_logits is not None:
+            raise ValueError("teacher= and teacher_logits= are two teachers; pass one")
+        if self.lsp is not None and aux is not None:
+            raise ValueError("aux= and the trainer's lsp= objective are two auxiliary losses; pass one")
+        if self.lsp is not None and teacher is None:
+            raise ValueError("the lsp= objective compares with the teacher's features: pass teacher=")
+        if teacher is not None:
+            self.check_teacher(teacher)
         self.forward(batch, x_dict, training=True)
         P = self._fwd["P"]
-        d_logits = self._loss(P, batch, teacher_logits)
-        d_feat = None
+        teacher_int = None
+        if teacher is not None:
+            teacher.forward(batch, x_dict, training=False, plan=P)
+            teacher_int = teacher._fwd["ys"][-1]
+        d_logits = self._loss(P, batch, teacher_logits, teacher_int)
+        d_feat = d_feat_int = None
         if aux is not None:
             d_feat, self.loss_aux = aux_grad(self.out_feat(), aux, beta)
-        dx0 = self.backward(d_logits, d_feat)
+        elif self.lsp is not None:
+            d_feat_int = self.lsp.forward_backward(self, teacher, batch)
+        dx0 = self.backward(d_logits, d_feat, d_feat_int)
         if self.emb:
             li = self._fwd["li_int"]
             order = device_argsort(P.node_type_int, li, self.T, max(self.num_nodes.values()))
@@ -496,6 +541,8 @@ class RGCNTrainer:
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
         if aux is not None:
             self.loss_out[0].add_(self.loss_aux * beta)
+        elif self.lsp is not None:
+            self.loss_out[2].copy_(self.lsp.loss_aux[0])
         return self.loss_out
 
     def gradients(self, batch, x_dict, d_logits: torch.Tensor) -> Dict[str, torch.Tensor]:

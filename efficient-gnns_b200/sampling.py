@@ -31,6 +31,38 @@ def random_walk(rowptr: torch.Tensor, col: torch.Tensor, start: torch.Tensor, wa
     return out
 
 
+def induced_edges(edge_index: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """The edges of ``edge_index`` [2, E] (int64, node ids of a batch) whose two endpoints are marked in ``mask`` [N] (bool),
+    relabelled to the endpoints' ranks among the marked nodes, edge order kept: ``torch_geometric.utils.subgraph(
+    mask.nonzero().squeeze(1), edge_index, relabel_nodes=True)[0]`` (the LSP edge list of mag_pyg/gnn_kd_and_aux.py:240-243),
+    element for element.  Scans and fill on the device (b200gnn_induced_edges_count / _fill_i64); one host read sizes the
+    output.  An edge with an endpoint outside [0, N) raises."""
+    if edge_index.dim() != 2 or edge_index.shape[0] != 2 or edge_index.dtype != torch.long or edge_index.stride(1) != 1:
+        raise lib.B200GnnError("induced_edges: edge_index must be an int64 [2, E] tensor with contiguous rows")
+    if mask.dim() != 1 or mask.dtype != torch.bool or not mask.is_contiguous():
+        raise lib.B200GnnError("induced_edges: mask must be a contiguous bool [N] tensor")
+    if not (edge_index.is_cuda and mask.is_cuda):
+        raise lib.B200GnnError("induced_edges: the edge list is built on the CUDA device; there is no CPU path")
+    L = lib.load()
+    dev = mask.device
+    n, E = mask.numel(), edge_index.shape[1]
+    ld = edge_index.stride(0)
+    rank = torch.empty(n + 1, dtype=torch.long, device=dev)
+    tiles = torch.empty(2 * max(int(L.b200gnn_induced_edges_tiles(E)), 1), dtype=torch.long, device=dev)
+    totals = torch.empty(2, dtype=torch.long, device=dev)
+    lib.check(L.b200gnn_induced_edges_count_i64(edge_index.data_ptr(), ld, E, mask.data_ptr(), n, rank.data_ptr(),
+                                                tiles.data_ptr(), totals.data_ptr(), lib.stream_ptr()), "induced_edges_count_i64")
+    kept, bad = totals.tolist()                              # the one host read of the batch: it sizes the output
+    if bad:
+        raise lib.B200GnnError(f"induced_edges: {bad} edges refer to a node outside the {n} of the mask")
+    out = torch.empty(2, kept, dtype=torch.long, device=dev)
+    if kept:
+        lib.check(L.b200gnn_induced_edges_fill_i64(edge_index.data_ptr(), ld, E, mask.data_ptr(), n, rank.data_ptr(),
+                                                   tiles.data_ptr(), out.data_ptr(), out.stride(0), lib.stream_ptr()),
+                  "induced_edges_fill_i64")
+    return out
+
+
 class SaintGraph:
     """CSR of the parent graph (rows = edge_index[0], as PyG's sampler builds its SparseTensor) + the parent edge id of every
     CSR position + the reusable node map."""

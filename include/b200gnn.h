@@ -837,6 +837,13 @@ int b200gnn_graph_coalesce_i64(const int64_t* row, const int64_t* col, int64_t n
  *   saint_subgraph: induced subgraph of the sorted unique node set `nodes` over CSR, CSR order kept.  count -> per selected
  *     row the number of kept edges (and fills node_map, an int32 [n_nodes] workspace that holds -1 on entry); the caller
  *     prefix-sums the counts into out_ptr; fill -> local row / local col / parent edge id (eid[j], or j when eid is NULL).
+ *   induced_edges: the edges of edge_index (int64 rows: src at edge_index[0..E), dst at edge_index[ld..ld+E)) whose two
+ *     endpoints are marked in mask (uint8 / bool [n_nodes]), relabelled to the endpoints' ranks among the marked nodes, edge
+ *     order kept: torch_geometric.utils.subgraph(mask.nonzero(), edge_index, relabel_nodes=True)[0].  count -> rank (int64
+ *     [n_nodes + 1] workspace: marked nodes before each node, rank[n_nodes] = all of them), tile_cnt (int64
+ *     [2 * b200gnn_induced_edges_tiles(E)] workspace) and totals (int64 [2]: kept edges, edges with an endpoint outside
+ *     [0, n_nodes), which are never kept); fill -> out[0..kept) sources and out[ld_out..ld_out + kept) destinations, reading
+ *     the rank and tile_cnt the count call left.
  * ------------------------------------------------------------------ */
 int b200gnn_random_walk_i64(const int32_t* rowptr, const int32_t* col, int64_t n_nodes, const int64_t* start,
                             int64_t n_walks, int32_t walk_length, uint64_t seed, uint64_t offset, int64_t* out,
@@ -846,6 +853,12 @@ int b200gnn_saint_subgraph_count_i64(const int32_t* rowptr, const int32_t* col, 
 int b200gnn_saint_subgraph_fill_i64(const int32_t* rowptr, const int32_t* col, const int64_t* eid, const int64_t* nodes,
                                     int64_t n_sel, const int32_t* node_map, const int64_t* out_ptr, int64_t* out_row,
                                     int64_t* out_col, int64_t* out_eid, void* stream);
+int64_t b200gnn_induced_edges_tiles(int64_t n_edges);
+int b200gnn_induced_edges_count_i64(const int64_t* edge_index, int64_t ld, int64_t n_edges, const uint8_t* mask,
+                                    int64_t n_nodes, int64_t* rank, int64_t* tile_cnt, int64_t* totals, void* stream);
+int b200gnn_induced_edges_fill_i64(const int64_t* edge_index, int64_t ld, int64_t n_edges, const uint8_t* mask,
+                                   int64_t n_nodes, const int64_t* rank, const int64_t* tile_cnt, int64_t* out,
+                                   int64_t ld_out, void* stream);
 
 #ifdef __cplusplus
 }
