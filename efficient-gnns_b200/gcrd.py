@@ -22,6 +22,9 @@ The sample cannot equal numpy's ``np.random.choice`` draw; ``train_step(..., sam
 
 ``PerGraphGCRD`` is the same objective for engine_ppi's PPI student, whose step trains on one whole graph at a time: the
 heads and the objective are GCRD's, the row set is the graph's n nodes.
+
+``BatchGCRD`` is the same objective for rgcn's MAG student on GraphSAINT batches, where the teacher's features and the
+number of train rows change with every batch: the row set is built per batch, on the sizes the step already holds.
 """
 from __future__ import annotations
 
@@ -30,7 +33,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import criterion, lib, ops
-from .heads import SAMPLE_STREAM, HeadRows, ProjectionHeads, _ceil4, _Pool, check_widths  # noqa: F401
+from .heads import SAMPLE_STREAM, HeadRows, ProjectionHeads, _ceil4, _Pool, check_sample, check_widths  # noqa: F401
 
 _EPS = 1e-12                                      # F.normalize
 
@@ -165,3 +168,98 @@ class PerGraphGCRD(GCRD):
         self._tail(r, feat)
         hi, lo = ops.split_tf32(self.W_s, transpose=True, hi=self.WsT_split[0], lo=self.WsT_split[1])
         ops.gemm_tf32x3(r.dz_s, hi, lo, out=d_feat)
+
+
+class BatchGCRD(GCRD):
+    """G-CRD inside rgcn.RGCNTrainer's step: the reference's MAG ``train()`` with ``--training nce``
+    (mag_pyg/gnn_kd_and_aux.py:258-271, 424-441) on every GraphSAINT batch b:
+
+        out_feat = student_proj(model.out_feat[b.train_mask])                      Linear(hidden, proj_dim), BN, ReLU
+        t_feat   = teacher_proj(teacher_model.out_feat[b.train_mask])              Linear(teacher hidden, proj_dim), BN, ReLU
+        loss_aux = nce_criterion(out, labels, out_feat, t_feat, beta, nce_T, max_samples)[2]
+        loss     = kd_criterion(out, labels, teacher_out, alpha, kd_T)[0] + beta * loss_aux
+        one Adam over the model and both heads
+
+    Per batch, between the student's loss and its backward (``RGCNTrainer(..., gcrd=g).train_step(b, x, teacher=t)``):
+
+        rows       a HeadRows for n = n_train rows and S = min(max_samples, n), its buffers from the caching allocator (the
+                   step is uncaptured and sized on the host); the sampler's workspace only when S < n
+        gather     G_t = the teacher's last hidden layer (eval: ReLU) and G_s = the student's (after ReLU and dropout) at the
+                   train rows, row k the k-th train row in batch order (as BatchLSP gathers them)
+        step       GCRD's draw (trainer seed, SAMPLE_STREAM, the student's device step counter), head front, objective, tail
+        d out_feat dz_s . W_s stored straight into a zeroed internal-order [N, H] gradient at the train rows
+
+    The trainer refuses a batch with one train row before any launch (the reference's BatchNorm1d raises ValueError).  A
+    batch with none does what the reference does: loss[0] and loss[2] are NaN, no head kernel runs (bn_finalize would write
+    NaN running statistics), the heads' gradients are zero and their Adam step is still taken (num_batches_tracked
+    advances), and the model's step is the KD step.  Parameters, Adam state, running statistics and state-dict I/O are
+    ProjectionHeads'."""
+
+    def __init__(self, hidden: int, teacher_hidden: int, proj_dim: int = 128, max_samples: int = 24576, nce_T: float = 0.075,
+                 beta: float = 0.1, seed: int = 0, bn_eps: float = 1e-5, bn_momentum: float = 0.1, device="cuda"):
+        """hidden / teacher_hidden: the student's and the teacher's last hidden widths (32 and 512 in the reference's MAG
+        models).  The defaults are the MAG script's (scripts/run_kd_and_aux.sh: beta 0.1, nce_T 0.075, max_samples 24576;
+        proj_dim 128 from argparse)."""
+        if int(max_samples) < 1:
+            raise ValueError("max_samples must be at least 1")
+        hidden, teacher_hidden = int(hidden), int(teacher_hidden)
+        check_widths(hidden, proj_dim, teacher_hidden)
+        self._init_heads(hidden, proj_dim, teacher_hidden, beta, seed, bn_eps, bn_momentum, torch.device(device))
+        self.nce_T, self.max_samples = float(nce_T), int(max_samples)
+        self.rows: Optional[HeadRows] = None                  # the last batch's row set
+        self.loss_aux = torch.full((1,), float("nan"), device=self.device)
+
+    def bind(self, trainer):
+        """Called by the RGCNTrainer that owns this object: its last hidden layer must be the width built for."""
+        if trainer.L < 2 or trainer.dims[-2] != self.H:
+            raise ValueError(f"G-CRD head built for hidden width {self.H}, the student's last hidden layer is "
+                             f"{trainer.dims[-2] if trainer.L >= 2 else 'absent'}")
+
+    def check_teacher(self, teacher):
+        """ValueError unless the teacher's last hidden layer has the width the teacher head was built for."""
+        if teacher.L < 2 or teacher.dims[-2] != self.F_t:
+            raise ValueError(f"G-CRD teacher head built for width {self.F_t}, the teacher's last hidden layer is "
+                             f"{teacher.dims[-2] if teacher.L >= 2 else 'absent'}")
+
+    def check_batch(self, n: int, sample=None):
+        """ValueError for a batch of n train rows the step cannot take (one row: BatchNorm has no variance), or a sample
+        that is not S = min(max_samples, n) distinct positions in [0, n)."""
+        if n == 1:
+            raise ValueError("a batch with one train row: the projection heads' BatchNorm needs more than one value per "
+                             "channel in training")
+        if sample is not None:
+            check_sample(sample, n, min(self.max_samples, n))
+
+    def sample(self) -> torch.Tensor:
+        """The last batch's sample: positions into its train rows (int64 [S])."""
+        return self.rows.inds.to(torch.int64) if self.rows is not None else torch.zeros(0, dtype=torch.int64)
+
+    def forward_backward(self, tr, teacher, sample: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+        """After tr's loss on its forward and teacher's eval forward on the same plan: returns d (beta * loss_aux) / d out_feat
+        [N, H] in internal row order (None when the batch has no train row) and adds beta * loss_aux to tr.loss_out[0]."""
+        f, dev = tr._fwd, self.device
+        train_int = f["train_int"]
+        n = train_int.numel()
+        if n == 0:
+            self.rows = None
+            self.grads.zero_()
+            self.loss_aux = torch.full((1,), float("nan"), device=dev)
+            tr.loss_out[:1].add_(self.loss_aux * self.beta)
+            return None
+        S, P = min(self.max_samples, n), self.P
+        feat_t = teacher._fwd["xs"][-1]
+        G_t = ops.gather_rows_act(feat_t, train_int, torch.empty(n, feat_t.shape[1], device=dev))
+        r = HeadRows(self, n, S, G_t, torch.zeros(_ceil4(S), P, device=dev), torch.zeros(_ceil4(S), P, device=dev),
+                     lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev))
+        self.rows, self.loss_aux = r, r.loss_aux
+        self.sample_ws = (torch.empty(int(lib.load().b200gnn_gcrd_sample_workspace_bytes(n)), dtype=torch.uint8, device=dev)
+                          if S < n else None)
+        self._draw(tr, r, sample)
+        G_s = ops.gather_rows_act(f["xs"][-1], train_int, torch.empty(n, self.H, device=dev))
+        self._front(r, G_s)
+        self._objective(tr, r)
+        self._tail(r, G_s)
+        d_feat = torch.zeros(f["P"].N, self.H, device=dev)
+        hi, lo = ops.split_tf32(self.W_s, transpose=True, hi=self.WsT_split[0], lo=self.WsT_split[1])
+        ops.gemm_tf32x3_rowidx(r.dz_s, hi, lo, d_feat, train_int)
+        return d_feat

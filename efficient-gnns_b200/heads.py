@@ -96,17 +96,22 @@ class HeadRows:
         heads._objective_buffers(self, alloc)
 
 
+def check_sample(sample, n: int, S: int) -> torch.Tensor:
+    """An injected sample as int64 [S] on the host; ValueError unless it holds S distinct positions in [0, n)."""
+    # the kernels index rows and store gradient rows by these positions: refuse what would go out of bounds or store one
+    # row twice (the override runs eagerly, so a host check costs nothing the step depends on)
+    s = torch.as_tensor(sample).to("cpu", torch.int64).view(-1)
+    if s.numel() != S or (S and (int(s.min()) < 0 or int(s.max()) >= n)) or s.unique().numel() != S:
+        raise ValueError(f"sample must hold {S} distinct positions in [0, {n})")
+    return s
+
+
 def draw_sample(tr, n: int, S: int, perm: torch.Tensor, workspace: Optional[torch.Tensor], sample: Optional[torch.Tensor]):
     """The step's sample of S of n rows into perm[:S] (int32 [n]): the injected ``sample``, or, when S < n, the on-device
     draw at (trainer seed, SAMPLE_STREAM, the trainer's device step counter) on ``workspace``
     (b200gnn_gcrd_sample_workspace_bytes(n) bytes).  Nothing when S = n and no sample is given."""
     if sample is not None:
-        # the kernels index rows and store gradient rows by these positions: refuse what would go out of bounds or store
-        # one row twice (the override runs eagerly, so a host check costs nothing the step depends on)
-        s = torch.as_tensor(sample).to("cpu", torch.int64).view(-1)
-        if s.numel() != S or (S and (int(s.min()) < 0 or int(s.max()) >= n)) or s.unique().numel() != S:
-            raise ValueError(f"sample must hold {S} distinct positions in [0, {n})")
-        perm[:S].copy_(s.to(torch.int32))
+        perm[:S].copy_(check_sample(sample, n, S).to(torch.int32))
     elif S < n:
         L = lib.load()
         lib.check(L.b200gnn_gcrd_sample_i32(n, tr.seed, SAMPLE_STREAM, lib.dptr(tr.step_count, torch.int32, "step"),

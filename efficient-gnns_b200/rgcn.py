@@ -29,7 +29,7 @@ import torch
 from . import lib, ops
 from .hybrid import DensePlan
 from .sparse import SparseTensor, csr_graph_from, device_argsort
-from .trainer import FlatParams, aux_grad
+from .trainer import FlatParams, aux_grad, one_objective
 
 
 def _block_plan(n: int, world: int) -> DensePlan:
@@ -266,8 +266,11 @@ class RGCNTrainer:
 
     def __init__(self, in_channels: int, hidden_channels: int, out_channels: int, num_layers: int, dropout: float,
                  num_nodes_dict: Dict[int, int], x_types, num_edge_types: int, relations: Dict[int, Tuple[int, int]],
-                 lr: float = 0.01, seed: int = 0, alpha: float = 0.9, kd_T: float = 4.0, device="cuda", lsp=None):
-        """lsp: an lsp.BatchLSP run inside every step (the reference's ``--training lpw``); its steps take ``teacher=``."""
+                 lr: float = 0.01, seed: int = 0, alpha: float = 0.9, kd_T: float = 4.0, device="cuda", lsp=None,
+                 gcrd=None):
+        """lsp: an lsp.BatchLSP run inside every step (the reference's ``--training lpw``); gcrd: a gcrd.BatchGCRD, the same
+        way (``--training nce``).  At most one of them; their steps take ``teacher=``."""
+        one_objective(gcrd=gcrd, lsp=lsp)
         self.dev = torch.device(device)
         self.F_in, self.H, self.C, self.L = int(in_channels), int(hidden_channels), int(out_channels), int(num_layers)
         self.p, self.lr, self.alpha, self.kd_T, self.seed = float(dropout), float(lr), float(alpha), float(kd_T), int(seed)
@@ -309,9 +312,10 @@ class RGCNTrainer:
         self.reset_parameters(seed)
         self._fwd = None
         self._training = False
-        self.lsp = lsp
-        if lsp is not None:
-            lsp.bind(self)
+        self.lsp, self.gcrd = lsp, gcrd
+        for o in (lsp, gcrd):
+            if o is not None:
+                o.bind(self)
 
     # ------------------------------------------------------------------ parameters
     def _wcatT(self, i: int, t: int, buf: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -502,23 +506,34 @@ class RGCNTrainer:
                                  "student's batch plan")
 
     def train_step(self, batch, x_dict: Dict[int, torch.Tensor], teacher_logits: Optional[torch.Tensor] = None, aux=None,
-                   beta: float = 1.0, teacher: Optional["RGCNTrainer"] = None) -> torch.Tensor:
+                   beta: float = 1.0, teacher: Optional["RGCNTrainer"] = None,
+                   sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One iteration of the reference ``train()`` loop body: logit-KD if ``teacher_logits`` ([n_train, C], the teacher's
         logits on the train_mask rows in batch order) or ``teacher`` is given, else cross-entropy, over the train_mask rows;
         then Adam over every parameter and embedding row.  ``aux(out_feat)`` as in ``GCNStudentTrainer.train_step``.
 
         ``teacher``: another RGCNTrainer (the reference's ``teacher_model``), run in eval mode on this step's batch plan (one
         plan per batch, no second sort); the KD loss reads its padded logits in place, and nothing of the teacher changes.
-        The trainer's ``lsp=`` objective needs it: the teacher's last hidden layer (ReLU, no dropout) is its feature side.
-        Returns the device tensor [loss, loss_cls, loss_kd] ([kd + beta * lsp, loss_cls, lsp] with lsp=)."""
+        The trainer's ``lsp=`` and ``gcrd=`` objectives need it: the teacher's last hidden layer (ReLU, no dropout) is their
+        feature side.  ``sample`` (positions into the batch's train rows, in batch order, [S]) replaces the gcrd= object's
+        on-device row sample (tests).  Returns the device tensor [loss, loss_cls, loss_kd] ([kd + beta * lsp, loss_cls, lsp]
+        with lsp=, [kd + beta * nce, loss_cls, nce] with gcrd=)."""
+        objective = self.lsp if self.lsp is not None else self.gcrd
+        name = "lsp=" if self.lsp is not None else "gcrd="
         if teacher is not None and teacher_logits is not None:
             raise ValueError("teacher= and teacher_logits= are two teachers; pass one")
-        if self.lsp is not None and aux is not None:
-            raise ValueError("aux= and the trainer's lsp= objective are two auxiliary losses; pass one")
-        if self.lsp is not None and teacher is None:
-            raise ValueError("the lsp= objective compares with the teacher's features: pass teacher=")
+        if objective is not None and aux is not None:
+            raise ValueError(f"aux= and the trainer's {name} objective are two auxiliary losses; pass one")
+        if objective is not None and teacher is None:
+            raise ValueError(f"the {name} objective compares with the teacher's features: pass teacher=")
+        if sample is not None and self.gcrd is None:
+            raise ValueError("sample= is the G-CRD row sample; this trainer has no gcrd= objective")
         if teacher is not None:
             self.check_teacher(teacher)
+        if self.gcrd is not None:
+            self.gcrd.check_teacher(teacher)
+            # the one host read of the train rows' count (the step reads the host anyway): refusals before any launch
+            self.gcrd.check_batch(int(batch.train_mask.sum()), sample)
         self.forward(batch, x_dict, training=True)
         P = self._fwd["P"]
         teacher_int = None
@@ -531,6 +546,8 @@ class RGCNTrainer:
             d_feat, self.loss_aux = aux_grad(self.out_feat(), aux, beta)
         elif self.lsp is not None:
             d_feat_int = self.lsp.forward_backward(self, teacher, batch)
+        elif self.gcrd is not None:
+            d_feat_int = self.gcrd.forward_backward(self, teacher, sample)
         dx0 = self.backward(d_logits, d_feat, d_feat_int)
         if self.emb:
             li = self._fwd["li_int"]
@@ -539,10 +556,12 @@ class RGCNTrainer:
                 ops.embedding_adam(dx0, P.node_type_int, li, order, t, e, self.emb_m[t], self.emb_v[t], self._head,
                                    self.step_count, self.lr)
         ops.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.step_count, self.lr)
+        if self.gcrd is not None:
+            self.gcrd.optimizer_step(self.lr)
         if aux is not None:
             self.loss_out[0].add_(self.loss_aux * beta)
-        elif self.lsp is not None:
-            self.loss_out[2].copy_(self.lsp.loss_aux[0])
+        elif objective is not None:
+            self.loss_out[2].copy_(objective.loss_aux[0])
         return self.loss_out
 
     def gradients(self, batch, x_dict, d_logits: torch.Tensor) -> Dict[str, torch.Tensor]:
