@@ -69,9 +69,11 @@ def _scaled(m: int, k: int, g: torch.Generator) -> torch.Tensor:
 
 
 def _bound_ratio(c: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
-    """max |c - ref| / bound (<= 1 passes); c fp32, ref / bound fp64, all on the GPU."""
+    """max |c - ref| / bound (<= 1 passes); c fp32, ref / bound fp64, all on the GPU.  An element whose bound is 0 (every
+    product of its dot product exactly zero, e.g. a dropped or ReLU-zero row of an activation) must equal ref exactly."""
     assert bool(torch.isfinite(c).all()), "non-finite output"
-    return float(((c.double() - ref).abs() / bound).max())
+    err = (c.double() - ref).abs()
+    return float(torch.where(bound > 0, err / bound, torch.where(err > 0, torch.inf, 0.0)).max())
 
 
 def _gemm_check(a, b, c, beta_, bias=None, c_in=None):
