@@ -322,50 +322,31 @@ class _GroupInput(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, node_type, local_node_idx, in_channels, keys, *tables):
-        import ctypes as C
         dev = node_type.device
         if not node_type.is_cuda:
             raise lib.B200GnnError("group_input: CUDA tensors only (no CPU fallback)")
-        n = node_type.numel()
         n_tables = (max(keys) + 1) if keys else 1
-        if n_tables > 16:
-            raise lib.B200GnnError("group_input: at most 16 node types")
-        ptrs = (C.c_void_p * n_tables)()
-        rows = (C.c_int64 * n_tables)()
-        for k, t in zip(keys, tables):
-            if t.dim() != 2 or t.shape[1] != in_channels or t.dtype != torch.float32 or not t.is_contiguous():
-                raise lib.B200GnnError(f"group_input: table of type {k} must be contiguous fp32 [rows, {in_channels}]")
-            ptrs[k], rows[k] = t.data_ptr(), t.shape[0]
-        out = torch.empty(n, in_channels, device=dev)
-        err = torch.zeros(1, dtype=torch.int32, device=dev)
-        nt, li = node_type.contiguous(), local_node_idx.contiguous()
-        lib.check(lib.load().b200gnn_typed_gather_f32(ptrs, rows, n_tables, nt.data_ptr(), li.data_ptr(), n, in_channels,
-                                                      out.data_ptr(), in_channels, err.data_ptr(), lib.stream_ptr()),
-                  "typed_gather_f32")
+        # the reference indexes with any integer tensor; the kernels read int64
+        nt, li = node_type.reshape(-1).long().contiguous(), local_node_idx.reshape(-1).long().contiguous()
+        out = torch.empty(nt.numel(), in_channels, device=dev)
+        ops.typed_gather(dict(zip(keys, tables)), n_tables, nt, li, out)   # raises on an index outside its table
         ctx.keys, ctx.shapes, ctx.n_tables = keys, [tuple(t.shape) for t in tables], n_tables
         ctx.save_for_backward(nt, li)
-        ctx.err = err
         return out
 
     @staticmethod
     def backward(ctx, d_out):
-        import ctypes as C
         nt, li = ctx.saved_tensors
-        n, F_ = d_out.shape
+        n = d_out.shape[0]
         needs = ctx.needs_input_grad[4:]
         grads = [torch.zeros(sh, device=d_out.device) if need else None for sh, need in zip(ctx.shapes, needs)]
         if any(needs) and n:
+            # every index of a type with a table is below big (the forward checked it); clamping the others, which the
+            # scatter skips, keeps their keys from landing inside a table type's run and splitting it in two
             big = int(max(sh[0] for sh in ctx.shapes)) + 1
-            order = torch.argsort(nt * big + li, stable=True)
-            ptrs = (C.c_void_p * ctx.n_tables)()
-            rows = (C.c_int64 * ctx.n_tables)()
-            for k, g, sh in zip(ctx.keys, grads, ctx.shapes):
-                rows[k] = sh[0]
-                if g is not None:
-                    ptrs[k] = g.data_ptr()
-            d = d_out.contiguous()
-            lib.check(lib.load().b200gnn_typed_scatter_f32(d.data_ptr(), d.stride(0), nt.data_ptr(), li.data_ptr(), order.data_ptr(),
-                                                           n, F_, ptrs, rows, ctx.n_tables, lib.stream_ptr()), "typed_scatter_f32")
+            order = torch.argsort(nt * big + li.clamp(0, big - 1), stable=True)
+            ops.typed_scatter(d_out.contiguous(), nt, li, order,
+                              {k: g for k, g in zip(ctx.keys, grads) if g is not None}, ctx.n_tables)
         return (None, None, None, None, *grads)
 
 

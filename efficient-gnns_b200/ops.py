@@ -571,30 +571,84 @@ def bn_act_bwd_apply(d_out, x_out, y, mean, invstd, gamma, sums, n_norm: int, p:
 def relu_dropout_bwd(d_out: torch.Tensor, x_out: torch.Tensor, p: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Backward of x_out = dropout_p(relu(y)): d_y = d_out * [x_out > 0] / (1-p) (contiguous [n, K]; out may be d_out)."""
     n, K = x_out.shape
-    assert d_out.shape == x_out.shape and d_out.is_contiguous() and x_out.is_contiguous()
     out = torch.empty_like(x_out) if out is None else out
+    if d_out.shape != x_out.shape or out.shape != x_out.shape:
+        raise lib.B200GnnError(f"relu_dropout_bwd: d_out {tuple(d_out.shape)} and out {tuple(out.shape)} must have the shape "
+                               f"of x_out {tuple(x_out.shape)}")
     lib.check(lib.load().b200gnn_relu_dropout_bwd_f32(_f32(d_out, "d_out"), _f32(x_out, "x_out"), _f32(out, "out"), n, K, float(p),
                                                       lib.stream_ptr()), "relu_dropout_bwd_f32")
     return out
 
 
-def _table_arrays(tables: dict, n_tables: int):
+MAX_TABLES = 16                         # Tables::ptr in csrc/hetero.cu
+
+
+def _table(t, name: str, F: int, dev: torch.device) -> None:
+    """The typed kernels index a table as fp32 rows of exactly F floats: anything else would be read as wrong rows."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != dev:
+        raise lib.B200GnnError(f"{name}: expected a CUDA tensor on {dev}")
+    if t.dtype != torch.float32 or t.dim() != 2 or not t.is_contiguous() or t.shape[1] != F:
+        raise lib.B200GnnError(f"{name}: expected a contiguous float32 [rows, {F}] table, got {t.dtype} "
+                               f"{tuple(t.shape)} with strides {t.stride()}")
+
+
+def _index(t, name: str, n: int, dev: torch.device) -> int:
+    """Device pointer of a contiguous int64 vector of length n (node types, local indices, sort orders)."""
+    if not isinstance(t, torch.Tensor) or t.dim() != 1 or t.numel() != n:
+        raise lib.B200GnnError(f"{name}: expected a 1-D int64 tensor of length {n}, got shape "
+                               f"{None if not isinstance(t, torch.Tensor) else tuple(t.shape)}")
+    if t.device != dev:
+        raise lib.B200GnnError(f"{name}: expected a tensor on {dev}, got {t.device}")
+    return lib.dptr(t, torch.int64, name)
+
+
+def _node_type_key(k, n_types: int, what: str) -> int:
+    import operator
+    try:
+        k = operator.index(k)
+    except TypeError:
+        raise lib.B200GnnError(f"{what} {k!r} is not an integer node type") from None
+    if not 0 <= k < n_types:
+        raise lib.B200GnnError(f"{what} {k} is not a node type in [0, {n_types})")
+    return k
+
+
+def _table_arrays(tables: dict, n_tables: int, F: int, dev: torch.device):
+    """Host arrays (pointer, rows) indexed by node type; types without a table get a null pointer."""
     import ctypes as C
+    if not 1 <= n_tables <= MAX_TABLES:
+        raise lib.B200GnnError(f"typed tables: n_tables = {n_tables}, the kernels take 1..{MAX_TABLES} node types")
     ptrs = (C.c_void_p * n_tables)()
     rows = (C.c_int64 * n_tables)()
     for k, t in tables.items():
+        k = _node_type_key(k, n_tables, "typed tables: key")
+        _table(t, f"table of type {k}", F, dev)
         ptrs[k], rows[k] = t.data_ptr(), t.shape[0]
     return ptrs, rows
 
 
 def typed_gather(tables: dict, n_tables: int, node_type: torch.Tensor, local_idx: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out[i] = tables[node_type[i]][local_idx[i]] (zero rows for types without a table); tables: {type: [rows, F] fp32}."""
-    ptrs, rows = _table_arrays(tables, n_tables)
+    """out[i] = tables[node_type[i]][local_idx[i]] (zero rows for types without a table); tables: {type: [rows, F] fp32}.
+
+    A local index outside its table raises B200GnnError naming the first such position, as the reference's indexing does.
+    Reading the kernel's error flag waits for the stream; the R-GCN step already reads the host while it builds its batch
+    plan, so this adds a wait but no new constraint (no caller captures the gather in a CUDA graph)."""
+    if not isinstance(out, torch.Tensor) or out.dim() != 2:
+        raise lib.B200GnnError("typed_gather: out must be a [n, F] tensor")
+    n, F_ = out.shape
+    ptrs, rows = _table_arrays(tables, n_tables, F_, out.device)
     err = torch.zeros(1, dtype=torch.int32, device=out.device)
-    lib.check(lib.load().b200gnn_typed_gather_f32(ptrs, rows, n_tables, lib.dptr(node_type, torch.int64, "node_type"),
-                                                  lib.dptr(local_idx, torch.int64, "local_idx"), out.shape[0], out.shape[1],
+    lib.check(lib.load().b200gnn_typed_gather_f32(ptrs, rows, n_tables, _index(node_type, "node_type", n, out.device),
+                                                  _index(local_idx, "local_idx", n, out.device), n, F_,
                                                   _f32(out, "out"), out.stride(0), err.data_ptr(), lib.stream_ptr()),
               "typed_gather_f32")
+    if int(err.item()):
+        bad = torch.zeros(n, dtype=torch.bool, device=out.device)
+        for k, t in tables.items():
+            bad |= (node_type == k) & ((local_idx < 0) | (local_idx >= t.shape[0]))
+        i = int(bad.nonzero()[0, 0])
+        raise lib.B200GnnError(f"typed_gather: local index {int(local_idx[i])} at position {i} is outside the "
+                               f"{tables[int(node_type[i])].shape[0]}-row table of node type {int(node_type[i])}")
     return out
 
 
@@ -602,10 +656,14 @@ def typed_scatter(d_out: torch.Tensor, node_type: torch.Tensor, local_idx: torch
                   n_tables: int) -> None:
     """grads[t][j] = sum of d_out[i] over nodes (node_type, local_idx) == (t, j), added in ``order`` (rows outside the batch are
     left untouched: pass zeroed tables for a dense gradient)."""
-    ptrs, rows = _table_arrays(grads, n_tables)
-    lib.check(lib.load().b200gnn_typed_scatter_f32(_f32(d_out, "d_out"), d_out.stride(0), lib.dptr(node_type, torch.int64, "node_type"),
-                                                   lib.dptr(local_idx, torch.int64, "local_idx"), lib.dptr(order, torch.int64, "order"),
-                                                   d_out.shape[0], d_out.shape[1], ptrs, rows, n_tables, lib.stream_ptr()),
+    if not isinstance(d_out, torch.Tensor) or d_out.dim() != 2:
+        raise lib.B200GnnError("typed_scatter: d_out must be a [n, F] tensor")
+    n, F_ = d_out.shape
+    ptrs, rows = _table_arrays(grads, n_tables, F_, d_out.device)
+    lib.check(lib.load().b200gnn_typed_scatter_f32(_f32(d_out, "d_out"), d_out.stride(0), _index(node_type, "node_type", n, d_out.device),
+                                                   _index(local_idx, "local_idx", n, d_out.device),
+                                                   _index(order, "order", n, d_out.device), n, F_, ptrs, rows, n_tables,
+                                                   lib.stream_ptr()),
               "typed_scatter_f32")
 
 
@@ -615,11 +673,24 @@ def embedding_adam(d_out: torch.Tensor, node_type: torch.Tensor, local_idx: torc
     """Adam over one embedding table whose gradient is typed_scatter(d_out) (``order``: the rows of d_out sorted by
     (node_type, local_idx)); bit-identical to the scatter into a zeroed dense gradient + adam_step, reads ``step`` without
     advancing it.  head: int32 [rows] scratch, all -1 (restored on return)."""
-    rows, F_ = table.shape
-    assert exp_avg.shape == table.shape == exp_avg_sq.shape and head.numel() >= rows and d_out.shape[1] == F_
+    if not isinstance(d_out, torch.Tensor) or d_out.dim() != 2:
+        raise lib.B200GnnError("embedding_adam: d_out must be a [n, F] tensor")
+    n, F_ = d_out.shape
+    dev = d_out.device
+    table_type = _node_type_key(table_type, MAX_TABLES, "embedding_adam: table_type")
+    for name, t in (("table", table), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _table(t, name, F_, dev)
+    rows = table.shape[0]
+    if exp_avg.shape != table.shape or exp_avg_sq.shape != table.shape:
+        raise lib.B200GnnError(f"embedding_adam: moments {tuple(exp_avg.shape)}, {tuple(exp_avg_sq.shape)} do not match the "
+                               f"table {tuple(table.shape)}")
+    if not isinstance(head, torch.Tensor) or head.dim() != 1 or head.numel() < rows or head.device != dev:
+        raise lib.B200GnnError(f"embedding_adam: head must be an int32 vector of at least {rows} entries on {dev}")
+    if not isinstance(step, torch.Tensor) or step.numel() != 1 or step.device != dev:
+        raise lib.B200GnnError(f"embedding_adam: step must be a one-element int32 tensor on {dev}")
     lib.check(lib.load().b200gnn_embedding_adam_f32(
-        _f32(d_out, "d_out"), d_out.stride(0), lib.dptr(node_type, torch.int64, "node_type"),
-        lib.dptr(local_idx, torch.int64, "local_idx"), lib.dptr(order, torch.int64, "order"), d_out.shape[0], int(table_type),
+        _f32(d_out, "d_out"), d_out.stride(0), _index(node_type, "node_type", n, dev), _index(local_idx, "local_idx", n, dev),
+        _index(order, "order", n, dev), n, table_type,
         _f32(table, "table"), _f32(exp_avg, "exp_avg"), _f32(exp_avg_sq, "exp_avg_sq"), rows, F_,
         lib.dptr(head, torch.int32, "head"), lr, betas[0], betas[1], eps, lib.dptr(step, torch.int32, "step"), lib.stream_ptr()),
         "embedding_adam_f32")
