@@ -1,6 +1,7 @@
 // Building blocks of the feature-distillation criteria of arxiv_pyg/criterion.py (fitnet :24-36, AT :39-54,
 // GSP/gpw :57-92, G-CRD/nce :129-149).  The S x S contractions themselves run on the wgmma GEMM
-// (gemm_tf32x3.cu); the kernels here are the row / element passes around them, each producing the forward value
+// (gemm_tf32x3.cu), except the narrow GSP contraction dG . x of a few-feature student (gsp_contract_kernel); the other
+// kernels here are the row / element passes around them, each producing the forward value
 // and the tensor the backward GEMM needs in the same pass.  Loss scalars are reduced deterministically
 // (per-CTA partials, fixed-order finalize).
 #include "common.cuh"
@@ -370,6 +371,117 @@ __global__ void __launch_bounds__(256) gsp_rows_backward_kernel(const int32_t* _
   if (loss_total && blockIdx.x == 0 && threadIdx.x == 0) loss_total[0] = __fadd_rn(loss_total[0], __fmul_rn(loss_aux[0], beta));
 }
 
+// ---------------------------------------------------------------- GSP: the narrow contraction g = dG . x
+// g[i, :F] = sum_{j<S} dG[i, j] x[j, :F] for a student side only a few features wide (F <= 128), where the 3xTF32 GEMM
+// would fill one 128 x 128 output tile per 128 rows.  The S columns are cut into slabs of GC_SLAB at absolute column
+// indices; a CTA takes GC_ROWS rows of one slab and walks it in tiles of GC_KT columns, ascending, accumulating in fp32
+// FMA.  The tiles are staged with cp.async into two buffers (dG rows into sG, x rows into sX), so the next tile's loads
+// run under this tile's FMAs.  A thread holds 4 rows x 4 features, so a CTA has 8 * F / 4 = 2F threads and
+// gsp_contract_smem(F) bytes of shared memory.  Each slab's partial goes to the workspace ([slab][row][F]) and
+// gsp_contract_reduce_kernel adds the slabs in ascending order; with one slab the CTA stores g itself.  So g[i] depends on
+// row i of dG and on x only: not on the chunk it sits in, the row count or the SM count.
+constexpr int GC_SLAB = B200GNN_GSP_CONTRACT_SLAB, GC_ROWS = 32, GC_KT = 32, GC_MAX_F = B200GNN_GSP_CONTRACT_MAX_F;
+constexpr int GC_SG = GC_ROWS * (GC_KT + 1);                 // floats of one sG buffer (row pitch 33: a warp's 4-row reads)
+
+__device__ __forceinline__ void gc_cp_async4(float* smem, const float* gmem) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(s), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void gc_cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void gc_cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+
+// column k of a thread's 4 rows (sG row pitch GC_KT + 1) times its 4 features of x row k (sX row pitch F)
+__device__ __forceinline__ void gsp_contract_step(float (&acc)[4][4], const float* sg, const float* sx, int k, int F) {
+  const float4 xv = *reinterpret_cast<const float4*>(sx + k * F);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float g = sg[q * (GC_KT + 1) + k];
+    acc[q][0] = fmaf(g, xv.x, acc[q][0]);
+    acc[q][1] = fmaf(g, xv.y, acc[q][1]);
+    acc[q][2] = fmaf(g, xv.z, acc[q][2]);
+    acc[q][3] = fmaf(g, xv.w, acc[q][3]);
+  }
+}
+
+__global__ void __launch_bounds__(256, 1) gsp_contract_kernel(const float* __restrict__ dG, int64_t ldg, int64_t n_rows, int S,
+                                                              const float* __restrict__ x, int64_t ldx, int F,
+                                                              float* __restrict__ out, int64_t ldo, int64_t slab_stride) {
+  extern __shared__ float4 gc_smem[];                        // two buffers of sX [GC_KT][F], then two of sG
+  float* sX = reinterpret_cast<float*>(gc_smem);
+  float* sG = sX + 2 * GC_KT * F;
+  const int tid = threadIdx.x, nthr = blockDim.x, fgs = F >> 2;
+  const int fg = tid % fgs, rg = tid / fgs;
+  const int64_t r0 = (int64_t)blockIdx.x * GC_ROWS;
+  const int j_begin = blockIdx.y * GC_SLAB, j_end = min(S, j_begin + GC_SLAB);
+  const int n_tiles = (j_end - j_begin + GC_KT - 1) / GC_KT;
+  // stage the columns [j0, j0 + kn) into buffer b: dG rows past n_rows and columns past kn are zero-filled, never read
+  auto stage = [&](int b, int j0) {
+    const int kn = min(GC_KT, j_end - j0);
+    float* g = sG + b * GC_SG;
+    for (int e = tid; e < GC_ROWS * GC_KT; e += nthr) {
+      const int r = e / GC_KT, k = e % GC_KT;
+      if (k < kn && r0 + r < n_rows) gc_cp_async4(g + r * (GC_KT + 1) + k, dG + (size_t)(r0 + r) * ldg + j0 + k);
+      else g[r * (GC_KT + 1) + k] = 0.f;
+    }
+    float* xs = sX + b * GC_KT * F;
+    for (int e = tid; e < kn * F; e += nthr) {
+      const int k = e / F, f = e - k * F;
+      gc_cp_async4(xs + k * F + f, x + (size_t)(j0 + k) * ldx + f);
+    }
+    gc_cp_async_commit();
+  };
+  float acc[4][4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[q][c] = 0.f;
+  stage(0, j_begin);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int j0 = j_begin + t * GC_KT, kn = min(GC_KT, j_end - j0), b = t & 1;
+    if (t + 1 < n_tiles) {
+      stage(b ^ 1, j0 + GC_KT);
+      gc_cp_async_wait<1>();
+    } else {
+      gc_cp_async_wait<0>();
+    }
+    __syncthreads();                                         // tile t is in buffer b for every thread
+    const float* g = sG + b * GC_SG + rg * 4 * (GC_KT + 1);
+    const float* xs = sX + b * GC_KT * F + fg * 4;
+    if (kn == GC_KT) {
+#pragma unroll
+      for (int k = 0; k < GC_KT; ++k) gsp_contract_step(acc, g, xs, k, F);
+    } else {
+      for (int k = 0; k < kn; ++k) gsp_contract_step(acc, g, xs, k, F);
+    }
+    __syncthreads();                                         // buffer b is refilled by tile t + 2
+  }
+  float* o = out + (size_t)blockIdx.y * slab_stride;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int64_t row = r0 + rg * 4 + q;
+    if (row < n_rows) {
+      float* orow = o + (size_t)row * ldo + fg * 4;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) orow[c] = acc[q][c];
+    }
+  }
+}
+
+static inline size_t gsp_contract_smem(int64_t F) { return (size_t)2 * (GC_KT * F + GC_SG) * sizeof(float); }
+
+// g[row, f] = the slabs' partials added in ascending slab order
+__global__ void __launch_bounds__(256) gsp_contract_reduce_kernel(const float* __restrict__ ws, int64_t n_rows, int F,
+                                                                  int slabs, float* __restrict__ g, int64_t ldo) {
+  const int64_t total = n_rows * (int64_t)F;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const float* p = ws + i;
+    float acc = p[0];
+    for (int s = 1; s < slabs; ++s) acc += p[(size_t)s * total];
+    g[(i / F) * ldo + i % F] = acc;
+  }
+}
+
 // F.binary_cross_entropy_with_logits(z, t) (ppi_pyg/criterion.py:11,13): element loss max(z,0) - z t + log1p(exp(-|z|)),
 // mean over all elements; d z = (sigmoid(z) - t) * w.  target_is_logits: t = sigmoid(target) (the teacher term of :13).
 __global__ void __launch_bounds__(256) bce_logits_kernel(const float* __restrict__ z, const float* __restrict__ target,
@@ -531,6 +643,60 @@ extern "C" int b200gnn_gsp_pair_chunk_f32(float* Gs, float* Gt, int64_t ld, int6
   const double n2 = (double)S * (double)S;
   gsp_pair_kernel<true><<<(int)n_rows, 256, 0, (cudaStream_t)stream>>>(Gs, Gt, ld, (int)S, (int)row_offset, ns, nt, kernel,
                                                                       (float)(2.0 / n2), rc_s, rc_t, partial);
+  return check_launch();
+}
+
+// The student side of b200gnn_gsp_pair_chunk_f32 alone: the same kernel, one-sided, so Gs, partial and (l2 / rbf) rc_s hold
+// the bits the two-sided pass stores for them; Gt is read only.  For a frozen teacher, whose gradient nobody reads.
+extern "C" int b200gnn_gsp_pair_student_chunk_f32(float* Gs, const float* Gt, int64_t ld, int64_t n_rows, int64_t S,
+                                                  int64_t row_offset, const float* ns, const float* nt, int kernel, float* rc_s,
+                                                  float* partial, void* stream) {
+  if (!Gs || !Gt || !partial || S <= 0 || S >= INT32_MAX || ld < S || n_rows <= 0 || row_offset < 0 ||
+      row_offset + n_rows > S || kernel < 0 || kernel > 3)
+    return B200GNN_ERR_BAD_ARG;
+  if (kernel >= 2 && (!ns || !nt || !rc_s)) return B200GNN_ERR_BAD_ARG;
+  const double n2 = (double)S * (double)S;
+  gsp_pair_kernel<false><<<(int)n_rows, 256, 0, (cudaStream_t)stream>>>(Gs, const_cast<float*>(Gt), ld, (int)S, (int)row_offset,
+                                                                       ns, nt, kernel, (float)(2.0 / n2), rc_s, nullptr,
+                                                                       partial);
+  return check_launch();
+}
+
+static inline int64_t gsp_contract_slabs(int64_t S) { return (S + GC_SLAB - 1) / GC_SLAB; }
+
+extern "C" size_t b200gnn_gsp_contract_workspace_bytes(int64_t n_rows, int64_t S, int64_t F) {
+  if (n_rows <= 0 || S <= 0 || F <= 0) return 0;
+  const int64_t slabs = gsp_contract_slabs(S);
+  return slabs > 1 ? (size_t)slabs * (size_t)n_rows * (size_t)F * sizeof(float) : 0;
+}
+
+// g[i, :F] (pitch ldo) = sum_{j<S} dG[i, j] x[j, :F] for the n_rows rows of dG (pitch ldg >= S; its columns S.. are not
+// read), x [S, F] at pitch ldx.  F a multiple of 4 up to 128.  workspace: b200gnn_gsp_contract_workspace_bytes bytes (none
+// when S fits one slab).
+extern "C" int b200gnn_gsp_contract_narrow_f32(const float* dG, int64_t ldg, int64_t n_rows, int64_t S, const float* x,
+                                               int64_t ldx, int64_t F, float* g, int64_t ldo, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
+  if (!dG || !x || !g || n_rows <= 0 || S <= 0 || F <= 0 || F % 4 || F > GC_MAX_F || ldg < S || ldx < F || ldo < F)
+    return B200GNN_ERR_BAD_ARG;
+  const int64_t slabs = gsp_contract_slabs(S), row_tiles = (n_rows + GC_ROWS - 1) / GC_ROWS;
+  if (slabs > 65535 || row_tiles > INT32_MAX) return B200GNN_ERR_BAD_ARG;
+  const size_t need = b200gnn_gsp_contract_workspace_bytes(n_rows, S, F);
+  if (need && (!workspace || workspace_bytes < need)) return B200GNN_ERR_BAD_ARG;
+  const void* al[] = {dG, x, g, workspace};
+  for (const void* p : al)
+    if (p && !aligned_to(p, 4)) return B200GNN_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = static_cast<float*>(workspace);
+  const dim3 grid((unsigned)row_tiles, (unsigned)slabs);
+  if (slabs == 1) {
+    gsp_contract_kernel<<<grid, (unsigned)(2 * F), gsp_contract_smem(F), st>>>(dG, ldg, n_rows, (int)S, x, ldx, (int)F, g, ldo, 0);
+    return check_launch();
+  }
+  int rc;
+  gsp_contract_kernel<<<grid, (unsigned)(2 * F), gsp_contract_smem(F), st>>>(dG, ldg, n_rows, (int)S, x, ldx, (int)F, ws, F,
+                                                                            n_rows * F);
+  if ((rc = check_launch())) return rc;
+  gsp_contract_reduce_kernel<<<ew_grid(n_rows * F), 256, 0, st>>>(ws, n_rows, (int)F, (int)slabs, g, ldo);
   return check_launch();
 }
 

@@ -25,6 +25,10 @@ injects one.
 
 ``PerGraphGSP`` is GSP for engine_ppi's PPI student, which has no heads: the loss compares the student's out_feat with the
 frozen teacher's, so each graph's teacher similarities are constants built once.
+
+``BatchGSP`` is GSP for rgcn.RGCNTrainer's MAG student on GraphSAINT batches, also without heads: per batch the teacher's
+last hidden layer comes from its eval forward on the student's plan, and the student's narrow gradient dG . x runs on the
+column-split contraction b200gnn_gsp_contract_narrow_f32 instead of the GEMM.
 """
 from __future__ import annotations
 
@@ -33,7 +37,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import criterion, lib, ops
-from .heads import ProjectionHeads, _ceil4, _Pool, draw_sample
+from .heads import ProjectionHeads, _ceil4, _Pool, check_sample, draw_sample
 
 _EPS = 1e-12                                      # F.normalize
 
@@ -265,3 +269,145 @@ class PerGraphGSP:
                                                   f(r.rc, "rc"), _EPS, self.beta, f(d_feat, "d_feat"), d_feat.stride(0),
                                                   f(r.loss_aux, "loss_aux"), f(tr.loss_out, "loss_out"), st),
                   "gsp_rows_backward_f32")
+
+
+class BatchGSP:
+    """GSP inside rgcn.RGCNTrainer's step: the reference's MAG ``train()`` with ``--training gpw``
+    (mag_pyg/gnn_kd_and_aux.py:229-242; criterion.py:57-92) on every GraphSAINT batch b, with no projection heads:
+
+        loss_aux = gpw_criterion(out, labels, model.out_feat[b.train_mask], teacher_model.out_feat[b.train_mask], kernel,
+                                 beta, max_samples)[2]              mean((sim_s - sim_t)^2) over S = min(max_samples, n) rows
+        loss     = kd_criterion(out, labels, teacher_out, alpha, kd_T)[0] + beta * loss_aux
+
+    Per batch, between the student's loss and its backward (``RGCNTrainer(..., gsp=o).train_step(b, x, teacher=t)``;
+    uncaptured, the buffers sized on the host from the batch's n):
+
+        rows         n = n_train, S = min(max_samples, n), Sp = S rounded up to 4
+        draw         only when S < n: G-CRD's sampler (trainer seed, SAMPLE_STREAM, the student's device step counter) into
+                     positions of the train rows, or the injected ``sample``; inds = train_int[perm[:S]] (int32 internal
+                     rows), or train_int itself when S = n
+        operands     b200gnn_gsp_rows_operands_f32 on the student's last hidden layer (after ReLU and dropout) and on the
+                     teacher's (its eval forward on the student's plan: ReLU, no dropout), read at inds in place
+        Gram chunks  per chunk of criterion.gsp_chunk_rows(Sp) rows, Gs_c = x_s[c] x_s^T and Gt_c = x_t[c] x_t^T on the
+                     3xTF32 GEMM, as criterion.gsp_chunks forms them
+        pair pass    b200gnn_gsp_pair_student_chunk_f32: d loss / d Gs_c in place, partial and (l2 / rbf) rc_s; the frozen
+                     teacher's gradient is never formed
+        contraction  b200gnn_gsp_contract_narrow_f32: g[c] = dGs_c . x_s in fp32 FMA over column slabs (the hidden width is
+                     narrow: one GEMM tile per 128 rows would leave the device idle)
+        finish       b200gnn_gsp_finish_f32
+        backward     b200gnn_gsp_rows_backward_f32 into a zeroed internal-order [N, H] gradient at inds, which the trainer
+                     adds at its last hidden layer; loss[0] += beta * loss_aux
+
+    The operands, the Gram GEMMs, the pair pass and the finish are the eager route's (``train_step(teacher_logits=...,
+    aux=lambda f: criterion.gpw_criterion(..., f[train_mask], t_feat[train_mask], kernel, 1, max_samples,
+    sampled_inds=...)[2], beta=beta)``), so loss_aux and loss[0] equal it bit for bit; only the contraction's sums run in
+    another order.  A batch with no train row does what the reference does: mse over nothing is NaN, so loss[0] and
+    loss[2] are NaN, no GSP kernel runs and the model takes the KD step.  One train row is a 1 x 1 problem whose two
+    similarities are equal: exactly for l2 and rbf (a row's distance to itself is 0), up to rounding for cosine and poly
+    (|x / |x||^2 = 1; a zero row normalises to zero on both sides), so the loss and the gradient are zero or rounding.
+    The reference's own loop refuses such a batch earlier, in cross_entropy (its labels.squeeze() leaves a 0-d target);
+    the trainer's KD step takes it.  No parameters, no optimizer state."""
+
+    NAME = "GSP"
+
+    def __init__(self, hidden: int, teacher_hidden: int, kernel: str = "poly", beta: float = 1.0, max_samples: int = 24576,
+                 device="cuda"):
+        """hidden / teacher_hidden: the student's and the teacher's last hidden widths (32 and 512 in the reference's MAG
+        models); hidden a multiple of 4 up to lib.GSP_CONTRACT_MAX_F, teacher_hidden a multiple of 4 up to
+        lib.GSP_ROWS_MAX_F.  The defaults are the MAG script's (scripts/run_kd_and_aux.sh runs gpw with kernel poly and
+        cosine, beta 1, max_samples 24576)."""
+        if kernel not in criterion._KERNELS:
+            raise ValueError(f"kernel {kernel!r}: GSP kernels are {sorted(criterion._KERNELS)}")
+        if int(max_samples) < 1:
+            raise ValueError("max_samples must be at least 1")
+        hidden, teacher_hidden = int(hidden), int(teacher_hidden)
+        if hidden % 4 or not 0 < hidden <= lib.GSP_CONTRACT_MAX_F:
+            raise ValueError(f"hidden width {hidden}: the narrow GSP contraction takes a multiple of 4 up to "
+                             f"{lib.GSP_CONTRACT_MAX_F}")
+        if teacher_hidden % 4 or not 0 < teacher_hidden <= lib.GSP_ROWS_MAX_F:
+            raise ValueError(f"teacher hidden width {teacher_hidden}: the GSP row passes take a multiple of 4 up to "
+                             f"{lib.GSP_ROWS_MAX_F}")
+        self.device = torch.device(device)
+        self.H, self.F_t, self.beta, self.max_samples = hidden, teacher_hidden, float(beta), int(max_samples)
+        self.kernel, self.kernel_id = kernel, criterion._KERNELS[kernel]
+        self.loss_aux = torch.full((1,), float("nan"), device=self.device)
+        self.inds: Optional[torch.Tensor] = None           # the last batch's sample: positions into its train rows
+
+    def bind(self, trainer):
+        """Called by the RGCNTrainer that owns this object: its last hidden layer must be the width built for."""
+        if trainer.L < 2 or trainer.dims[-2] != self.H:
+            raise ValueError(f"GSP built for hidden width {self.H}, the student's last hidden layer is "
+                             f"{trainer.dims[-2] if trainer.L >= 2 else 'absent'}")
+
+    def check_teacher(self, teacher):
+        """ValueError unless the teacher's last hidden layer has the width built for."""
+        if teacher.L < 2 or teacher.dims[-2] != self.F_t:
+            raise ValueError(f"GSP built for teacher hidden width {self.F_t}, the teacher's last hidden layer is "
+                             f"{teacher.dims[-2] if teacher.L >= 2 else 'absent'}")
+
+    def check_batch(self, n: int, sample=None):
+        """ValueError for a sample that is not S = min(max_samples, n) distinct positions in [0, n), or any sample when
+        S = n (every train row is taken; there is nothing to draw)."""
+        if sample is None:
+            return
+        S = min(self.max_samples, n)
+        if S == n:
+            raise ValueError(f"GSP takes every train row of this batch (max_samples {self.max_samples} >= {n}): there is "
+                             "no sample to inject")
+        check_sample(sample, n, S)
+
+    def sample(self) -> torch.Tensor:
+        """The last batch's sample: positions into its train rows (int64 [S])."""
+        return self.inds.to(torch.int64) if self.inds is not None else torch.zeros(0, dtype=torch.int64)
+
+    def forward_backward(self, tr, teacher, sample: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+        """After tr's loss on its forward and teacher's eval forward on the same plan: returns d (beta * loss_aux) / d out_feat
+        [N, H] in internal row order (None when the batch has no train row) and adds beta * loss_aux to tr.loss_out[0]."""
+        f, dev = tr._fwd, self.device
+        train_int = f["train_int"]
+        n = train_int.numel()
+        if n == 0:
+            self.inds = None
+            self.loss_aux = torch.full((1,), float("nan"), device=dev)
+            tr.loss_out[:1].add_(self.loss_aux * self.beta)
+            return None
+        S, H, Ft, k = min(self.max_samples, n), self.H, self.F_t, self.kernel_id
+        Sp, raw = _ceil4(S), k >= 2
+        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)     # noqa: E731
+        perm = torch.arange(n, dtype=torch.int32, device=dev)
+        ws = (torch.empty(int(lib.load().b200gnn_gcrd_sample_workspace_bytes(n)), dtype=torch.uint8, device=dev)
+              if S < n and sample is None else None)
+        draw_sample(tr, n, S, perm, ws, sample)
+        self.inds = perm[:S]
+        rows = (train_int[perm[:S].long()] if S < n else train_int).to(torch.int32)
+        L, st = lib.load(), lib.stream_ptr()
+        fp = lambda t, name: lib.dptr(t, torch.float32, name)      # noqa: E731
+        # operands, zero-padded to Sp rows (the Gram GEMMs read all Sp rows of x as their B operand)
+        x_s, x_t = torch.zeros(Sp, H, device=dev), torch.zeros(Sp, Ft, device=dev)
+        norm_s, norm_t = e(Sp), e(Sp)
+        for feat, x, nrm, F, name in ((f["xs"][-1], x_s, norm_s, H, "student"),
+                                      (teacher._fwd["xs"][-1], x_t, norm_t, Ft, "teacher")):
+            lib.check(L.b200gnn_gsp_rows_operands_f32(fp(feat, name), feat.stride(0), rows.data_ptr(), S, F, k, _EPS,
+                                                      fp(x, "x"), F, fp(nrm, "norm"), st), "gsp_rows_operands_f32")
+        hs, ls = ops.split_tf32(x_s)
+        ht, lt = ops.split_tf32(x_t)
+        R = criterion.gsp_chunk_rows(Sp)
+        Gs, Gt = e(R, Sp), e(R, Sp)
+        rc_s, part, g, loss = (e(Sp) if raw else None), e(Sp), e(Sp, H), e(1)
+        cws = ops.gsp_contract_workspace(min(R, S), S, H, dev)
+        for r0 in range(0, S, R):
+            r = min(R, S - r0)
+            ops.gemm_tf32x3(x_s[r0:r0 + r], hs, ls, out=Gs[:r])
+            ops.gemm_tf32x3(x_t[r0:r0 + r], ht, lt, out=Gt[:r])
+            lib.check(L.b200gnn_gsp_pair_student_chunk_f32(fp(Gs, "Gs"), fp(Gt, "Gt"), Sp, r, S, r0,
+                                                           fp(norm_s if raw else None, "ns"), fp(norm_t if raw else None, "nt"),
+                                                           k, fp(rc_s, "rc_s"), fp(part, "part"), st),
+                      "gsp_pair_student_chunk_f32")
+            ops.gsp_contract_narrow(Gs[:r], S, x_s, g[r0:r0 + r], cws)
+        lib.check(L.b200gnn_gsp_finish_f32(fp(part, "part"), S, fp(loss, "loss"), st), "gsp_finish_f32")
+        self.loss_aux = loss
+        d_feat = torch.zeros(f["P"].N, H, device=dev)
+        lib.check(L.b200gnn_gsp_rows_backward_f32(rows.data_ptr(), S, H, k, fp(g, "g"), fp(x_s, "x_s"), H, fp(norm_s, "norm"),
+                                                  fp(rc_s, "rc"), _EPS, self.beta, fp(d_feat, "d_feat"), H, fp(loss, "loss_aux"),
+                                                  fp(tr.loss_out, "loss_out"), st), "gsp_rows_backward_f32")
+        return d_feat

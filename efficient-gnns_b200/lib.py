@@ -19,6 +19,8 @@ REDUCE_SUM = 0
 REDUCE_MEAN = 1
 LSP_MAX_F = 512          # B200GNN_LSP_MAX_F: widest student row b200gnn_lsp_student_f32 holds in registers
 GSP_ROWS_MAX_F = 2048    # B200GNN_GSP_ROWS_MAX_F: widest feature row of the fixed-teacher GSP row passes
+GSP_CONTRACT_MAX_F = 128  # B200GNN_GSP_CONTRACT_MAX_F: widest student side of the narrow GSP contraction
+GSP_CONTRACT_SLAB = 256   # B200GNN_GSP_CONTRACT_SLAB: its column slab
 
 _i32p = C.c_void_p
 _f32p = C.c_void_p
@@ -141,6 +143,11 @@ SIGNATURES = {
     "b200gnn_gsp_pair_f32": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _int, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_gsp_pair_chunk_f32": (_int, [_f32p, _f32p, _i64, _i64, _i64, _i64, _f32p, _f32p, _int, _f32p, _f32p, _f32p, _ptr]),
     "b200gnn_gsp_finish_f32": (_int, [_f32p, _i64, _f32p, _ptr]),
+    "b200gnn_gsp_pair_student_chunk_f32": (_int, [_f32p, _f32p, _i64, _i64, _i64, _i64, _f32p, _f32p, _int, _f32p, _f32p,
+                                                  _ptr]),
+    "b200gnn_gsp_contract_workspace_bytes": (C.c_size_t, [_i64, _i64, _i64]),
+    "b200gnn_gsp_contract_narrow_f32": (_int, [_f32p, _i64, _i64, _i64, _f32p, _i64, _i64, _f32p, _i64, _ptr, C.c_size_t,
+                                               _ptr]),
     "b200gnn_gsp_operands_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _f32p, _f32, _f32p, _f32p, _f32p, _f32p,
                                         _ptr]),
     "b200gnn_gsp_backward_f32": (_int, [_i32p, _i64, _i64, _int, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32,

@@ -285,6 +285,29 @@ def scatter_rows_scaled(src: torch.Tensor, idx: torch.Tensor, scale: float, out:
     return out
 
 
+def gsp_contract_workspace(n_rows: int, S: int, F: int, device) -> Optional[torch.Tensor]:
+    """The workspace gsp_contract_narrow needs for n_rows rows (None when S fits one slab)."""
+    nbytes = int(lib.load().b200gnn_gsp_contract_workspace_bytes(n_rows, S, F))
+    return torch.empty(nbytes, dtype=torch.uint8, device=device) if nbytes else None
+
+
+def gsp_contract_narrow(dG: torch.Tensor, S: int, x: torch.Tensor, out: torch.Tensor,
+                        workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[i, :F] = sum_{j<S} dG[i, j] x[j, :F] in fp32 FMA (b200gnn_gsp_contract_narrow_f32): dG [n_rows, >= S] rows at a
+    row pitch, x [>= S, F] with F a multiple of 4 up to lib.GSP_CONTRACT_MAX_F, out [n_rows, F] at a row pitch.  Row i of
+    out depends on row i of dG and on x only.  workspace: gsp_contract_workspace(n_rows, S, F) or larger."""
+    n_rows, F = dG.shape[0], x.shape[1]
+    assert out.shape[0] == n_rows and out.shape[1] == F and x.shape[0] >= S
+    for t, name in ((dG, "dG"), (x, "x"), (out, "out")):
+        if t.dtype != torch.float32 or not t.is_cuda or t.stride(1) != 1:
+            raise lib.B200GnnError(f"gsp_contract_narrow: {name} must be float32 CUDA rows with unit column stride")
+    ws = 0 if workspace is None else workspace.numel() * workspace.element_size()
+    lib.check(lib.load().b200gnn_gsp_contract_narrow_f32(
+        dG.data_ptr(), dG.stride(0), n_rows, int(S), x.data_ptr(), x.stride(0), F, out.data_ptr(), out.stride(0),
+        None if workspace is None else workspace.data_ptr(), ws, lib.stream_ptr()), "gsp_contract_narrow_f32")
+    return out
+
+
 def bn_act_bwd(d_out, x_out, y, mean, invstd, gamma, p: float, d_y=None, d_gamma=None, d_beta=None, d_bias=None,
                partial=None, coef=None, want_dbias: bool = True):
     """Backward of x_out = dropout_p(relu(BN_train(y))). Returns (d_y, d_gamma, d_beta, d_bias)."""

@@ -267,10 +267,11 @@ class RGCNTrainer:
     def __init__(self, in_channels: int, hidden_channels: int, out_channels: int, num_layers: int, dropout: float,
                  num_nodes_dict: Dict[int, int], x_types, num_edge_types: int, relations: Dict[int, Tuple[int, int]],
                  lr: float = 0.01, seed: int = 0, alpha: float = 0.9, kd_T: float = 4.0, device="cuda", lsp=None,
-                 gcrd=None):
+                 gcrd=None, gsp=None):
         """lsp: an lsp.BatchLSP run inside every step (the reference's ``--training lpw``); gcrd: a gcrd.BatchGCRD, the same
-        way (``--training nce``).  At most one of them; their steps take ``teacher=``."""
-        one_objective(gcrd=gcrd, lsp=lsp)
+        way (``--training nce``); gsp: a gsp.BatchGSP (``--training gpw``).  At most one of them; their steps take
+        ``teacher=``."""
+        one_objective(gcrd=gcrd, lsp=lsp, gsp=gsp)
         self.dev = torch.device(device)
         self.F_in, self.H, self.C, self.L = int(in_channels), int(hidden_channels), int(out_channels), int(num_layers)
         self.p, self.lr, self.alpha, self.kd_T, self.seed = float(dropout), float(lr), float(alpha), float(kd_T), int(seed)
@@ -312,8 +313,8 @@ class RGCNTrainer:
         self.reset_parameters(seed)
         self._fwd = None
         self._training = False
-        self.lsp, self.gcrd = lsp, gcrd
-        for o in (lsp, gcrd):
+        self.lsp, self.gcrd, self.gsp = lsp, gcrd, gsp
+        for o in (lsp, gcrd, gsp):
             if o is not None:
                 o.bind(self)
 
@@ -514,26 +515,30 @@ class RGCNTrainer:
 
         ``teacher``: another RGCNTrainer (the reference's ``teacher_model``), run in eval mode on this step's batch plan (one
         plan per batch, no second sort); the KD loss reads its padded logits in place, and nothing of the teacher changes.
-        The trainer's ``lsp=`` and ``gcrd=`` objectives need it: the teacher's last hidden layer (ReLU, no dropout) is their
-        feature side.  ``sample`` (positions into the batch's train rows, in batch order, [S]) replaces the gcrd= object's
-        on-device row sample (tests).  Returns the device tensor [loss, loss_cls, loss_kd] ([kd + beta * lsp, loss_cls, lsp]
-        with lsp=, [kd + beta * nce, loss_cls, nce] with gcrd=)."""
-        objective = self.lsp if self.lsp is not None else self.gcrd
-        name = "lsp=" if self.lsp is not None else "gcrd="
+        The trainer's ``lsp=``, ``gcrd=`` and ``gsp=`` objectives need it: the teacher's last hidden layer (ReLU, no dropout)
+        is their feature side.  ``sample`` (positions into the batch's train rows, in batch order, [S]) replaces the gcrd= or
+        gsp= object's on-device row sample (tests).  Returns the device tensor [loss, loss_cls, loss_kd] ([kd + beta * lsp,
+        loss_cls, lsp] with lsp=, [kd + beta * nce, loss_cls, nce] with gcrd=, [kd + beta * gsp, loss_cls, gsp] with gsp=)."""
+        objective = one_objective(gcrd=self.gcrd, lsp=self.lsp, gsp=self.gsp)
+        name = "lsp=" if self.lsp is not None else "gcrd=" if self.gcrd is not None else "gsp="
         if teacher is not None and teacher_logits is not None:
             raise ValueError("teacher= and teacher_logits= are two teachers; pass one")
         if objective is not None and aux is not None:
             raise ValueError(f"aux= and the trainer's {name} objective are two auxiliary losses; pass one")
         if objective is not None and teacher is None:
             raise ValueError(f"the {name} objective compares with the teacher's features: pass teacher=")
-        if sample is not None and self.gcrd is None:
-            raise ValueError("sample= is the G-CRD row sample; this trainer has no gcrd= objective")
+        if sample is not None and self.gcrd is None and self.gsp is None:
+            raise ValueError("sample= is the G-CRD / GSP row sample; this trainer has no gcrd= objective and no gsp= "
+                             "objective")
         if teacher is not None:
             self.check_teacher(teacher)
         if self.gcrd is not None:
             self.gcrd.check_teacher(teacher)
             # the one host read of the train rows' count (the step reads the host anyway): refusals before any launch
             self.gcrd.check_batch(int(batch.train_mask.sum()), sample)
+        if self.gsp is not None:
+            self.gsp.check_teacher(teacher)
+            self.gsp.check_batch(int(batch.train_mask.sum()), sample)
         self.forward(batch, x_dict, training=True)
         P = self._fwd["P"]
         teacher_int = None
@@ -548,6 +553,8 @@ class RGCNTrainer:
             d_feat_int = self.lsp.forward_backward(self, teacher, batch)
         elif self.gcrd is not None:
             d_feat_int = self.gcrd.forward_backward(self, teacher, sample)
+        elif self.gsp is not None:
+            d_feat_int = self.gsp.forward_backward(self, teacher, sample)
         dx0 = self.backward(d_logits, d_feat, d_feat_int)
         if self.emb:
             li = self._fwd["li_int"]

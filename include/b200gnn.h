@@ -529,6 +529,22 @@ int b200gnn_gsp_pair_chunk_f32(float* Gs, float* Gt, int64_t ld, int64_t n_rows,
                                const float* ns, const float* nt, int kernel, float* rc_s, float* rc_t, float* partial,
                                void* stream);
 int b200gnn_gsp_finish_f32(const float* partial, int64_t S, float* loss_out, void* stream);
+/* The student side of b200gnn_gsp_pair_chunk_f32 alone (a frozen teacher: Gt is read, never written; no rc_t): Gs,
+ * partial and (kernels 2,3) rc_s hold the bits the two-sided pass stores for them. */
+int b200gnn_gsp_pair_student_chunk_f32(float* Gs, const float* Gt, int64_t ld, int64_t n_rows, int64_t S, int64_t row_offset,
+                                       const float* ns, const float* nt, int kernel, float* rc_s, float* partial,
+                                       void* stream);
+/* The narrow GSP contraction (csrc/loss_pair.cu): g[i, :F] (pitch ldo) = sum_{j<S} dG[i, j] x[j, :F] for the n_rows rows of
+ * dG (pitch ldg >= S; columns S.. are not read) and x [S, F] (pitch ldx), in fp32 FMA.  F is a multiple of 4 up to
+ * B200GNN_GSP_CONTRACT_MAX_F.  The columns are summed in slabs of B200GNN_GSP_CONTRACT_SLAB at absolute column indices,
+ * ascending within a slab, and the slabs' partials are added in ascending order, so g[i] depends only on row i of dG and
+ * on x (not on n_rows, the chunk a row sits in, or the device).  workspace: at least
+ * b200gnn_gsp_contract_workspace_bytes(n_rows, S, F) bytes (0 when S fits one slab: workspace may be null). */
+#define B200GNN_GSP_CONTRACT_MAX_F 128
+#define B200GNN_GSP_CONTRACT_SLAB 256
+size_t b200gnn_gsp_contract_workspace_bytes(int64_t n_rows, int64_t S, int64_t F);
+int b200gnn_gsp_contract_narrow_f32(const float* dG, int64_t ldg, int64_t n_rows, int64_t S, const float* x, int64_t ldx,
+                                    int64_t F, float* g, int64_t ldo, void* workspace, size_t workspace_bytes, void* stream);
 /* The captured GSP step (csrc/gcrd.cu; gpw_criterion :57-92 on the projection heads of the G-CRD step).
  *   gsp_operands: kernel 0 cosine / 1 poly: x_*[j] = relu(bn_*(pre_*[inds[j]])) normalised (F.normalize, eps), its norm to
  *     norm_*[j]; kernel 2 l2 / 3 rbf: x_*[j] = relu(bn_*(pre_*[inds[j]])) and its squared norm to norm_*[j].
