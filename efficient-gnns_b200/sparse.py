@@ -125,15 +125,22 @@ def _on_engine_device(*ts) -> bool:
 
 
 def device_argsort(major: torch.Tensor, minor: torch.Tensor, major_size: int, minor_size: int) -> torch.Tensor:
-    """Stable argsort of major*minor_size + minor: the hand-written radix sort on CUDA tensors (int64 in, int64 out, same
-    permutation as torch.argsort(stable=True)); torch on CPU tensors (host-side logic and its tests)."""
+    """Stable argsort of major*minor_size + minor: the hand-written radix sort on CUDA tensors (int64 out, same
+    permutation as torch.argsort(stable=True)); torch on CPU tensors (host-side logic and its tests).  The CPU order is two
+    stable passes, minor then major, so that key ranges of 2^63 and above (which the radix sort accepts) do not overflow."""
     n = int(major.numel())
-    if n == 0 or not _on_engine_device(major, minor) or n >= 2 ** 31 - 1 or float(major_size) * float(minor_size) >= 1.8e19:
-        return torch.argsort(major * minor_size + minor, stable=True)
+    if not _on_engine_device(major, minor):
+        p = torch.argsort(minor, stable=True)
+        return p[torch.argsort(major[p], stable=True)]
+    if n == 0:
+        return torch.empty(0, dtype=torch.long, device=major.device)
+    if n >= 2 ** 31 - 1 or float(major_size) * float(minor_size) >= 1.8e19:
+        raise lib.B200GnnError(f"device_argsort: {n} keys in a range of {major_size} x {minor_size}: the radix sort takes fewer "
+                               "than 2^31-1 keys and a key range below 1.8e19")
     L = lib.load()
     ws = torch.empty(int(L.b200gnn_graph_sort_workspace_bytes(n)), dtype=torch.uint8, device=major.device)
     perm = torch.empty(n, dtype=torch.int32, device=major.device)
-    ma, mi = major.contiguous(), minor.contiguous()
+    ma, mi = major.to(torch.long).contiguous(), minor.to(torch.long).contiguous()     # the kernel reads int64
     lib.check(L.b200gnn_graph_argsort_i64(ma.data_ptr(), mi.data_ptr(), n, int(major_size), int(minor_size), perm.data_ptr(),
                                           ws.data_ptr(), lib.stream_ptr()), "graph_argsort_i64")
     return perm.long()
@@ -149,7 +156,7 @@ def device_coalesce(row: torch.Tensor, col: torch.Tensor, n_rows: int, n_cols: i
     src = torch.empty(n, dtype=torch.int32, device=dev)
     rowptr = torch.empty(n_rows + 1, dtype=torch.long, device=dev)
     nnz = torch.zeros(1, dtype=torch.long, device=dev)
-    r, c = row.contiguous(), col.contiguous()
+    r, c = row.to(torch.long).contiguous(), col.to(torch.long).contiguous()     # the kernel reads int64
     lib.check(L.b200gnn_graph_coalesce_i64(r.data_ptr(), c.data_ptr(), n, int(n_rows), int(n_cols), out_row.data_ptr(),
                                            out_col.data_ptr(), src.data_ptr(), rowptr.data_ptr(), nnz.data_ptr(), ws.data_ptr(),
                                            lib.stream_ptr()), "graph_coalesce_i64")
