@@ -184,7 +184,10 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   constexpr bool XYTMA = STAT == 3;
   constexpr bool COLSTAT = STAT >= 1 && STAT <= 3;   // per-column reductions in the statistics block
   constexpr bool PRB = STAT == 4;                    // PReLU/dropout backward epilogue
-  constexpr bool PRO = (ACT || PRELU) && !STAT;      // activation prologue on A (keep words fetched a stage ahead)
+  // PReLU prologue: register-only (keep words from global memory, one slope scalar), so it also runs under the statistics
+  // epilogue (STAT == 1: the SIGN G-CRD student head); ACT keeps its (scale, shift) table in the statistics block
+  constexpr bool PRO_PRELU = PRELU && (STAT == 0 || STAT == 1);
+  constexpr bool PRO = (ACT && !STAT) || PRO_PRELU;  // activation prologue on A (keep words fetched a stage ahead)
   constexpr int BN = C::BN, STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, B_TILE_BYTES = C::B_TILE_BYTES, ACC = C::ACC;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -316,7 +319,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                            p.inv_keep);
         }
       }
-      if (PRELU && !STAT) {
+      if (PRO_PRELU) {
 #pragma unroll
         for (int k = 0; k < BK / 8; ++k)
 #pragma unroll
@@ -618,6 +621,13 @@ static int gemm_dispatch(const float* A, int64_t lda, const float* B_hi, const f
   if (prelu) {
     if (!prelu->act_slope || !prelu->act_bits) return B200GNN_ERR_BAD_ARG;
     p.act_slope = prelu->act_slope; p.act_bits = prelu->act_bits; p.act_words = prelu->act_words; p.inv_keep = prelu->inv_keep;
+    if (prelu->stat_mode == 0 && st) {
+      // PReLU prologue with the BatchNorm statistics epilogue: the refusals of the statistics GEMM
+      if (st->stat_mode != 1 || N % 32 || N > gemm::STAT_MAX_N || N <= 48 || ldc % 4 || !aligned_to(C, 16) || !st->stat_partial)
+        return B200GNN_ERR_UNSUPPORTED;
+      p.stat_mode = 1; p.stat_partial = st->stat_partial;
+      return gemm::launch<gemm::Cfg<128, 4>, 1, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
+    }
     if (prelu->stat_mode == 0) {
       if (N <= 48) return gemm::launch<gemm::Cfg<48, 6>, 0, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
       return gemm::launch<gemm::Cfg<128, 4>, 0, false, false, true>(A, lda, B_hi, B_lo, ldb, p, (cudaStream_t)stream);
@@ -733,6 +743,22 @@ extern "C" int b200gnn_gemm_tf32x3_prelu_f32(const float* Z, int64_t lda, const 
   pr.stat_mode = 0; pr.act_slope = slope; pr.act_bits = bits; pr.act_words = (int32_t)((K + 31) / 32);
   pr.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
   return gemm_dispatch(Z, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, bias, 0, stream, nullptr, nullptr, &pr);
+}
+
+// b200gnn_gemm_tf32x3_prelu_f32 with the BatchNorm batch statistics of C taken in the epilogue, as
+// b200gnn_gemm_tf32x3_stats_f32 takes them: output and partial[slots][2][N] are bit for bit those of the statistics GEMM on
+// the activation b200gnn_prelu_bits_f32 materialises (the SIGN G-CRD student head, Linear(hops * hidden, proj_dim) -> BN,
+// reading the concatenation without storing dropout(prelu(cat))).  N a multiple of 32 in (48, 256].
+extern "C" int b200gnn_gemm_tf32x3_prelu_stats_f32(const float* Z, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                                   float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                                   const float* slope, const uint32_t* bits, float p_drop, float* partial,
+                                                   int64_t slots, void* stream) {
+  if (p_drop < 0.f || p_drop >= 1.f || !partial || slots < b200gnn_gemm_stat_slots(M, N)) return B200GNN_ERR_BAD_ARG;
+  gemm::Params st{}, pr{};
+  st.stat_mode = 1; st.stat_partial = partial;
+  pr.stat_mode = 0; pr.act_slope = slope; pr.act_bits = bits; pr.act_words = (int32_t)((K + 31) / 32);
+  pr.inv_keep = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
+  return gemm_dispatch(Z, lda, B_hi, B_lo, ldb, C, ldc, M, N, K, bias, 0, stream, &st, nullptr, &pr);
 }
 
 // The input-gradient GEMM behind x = dropout(prelu(Z)): dA = A · B^T (+ C when accumulate); what is STORED to C is

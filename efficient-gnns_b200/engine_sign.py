@@ -15,9 +15,15 @@ One step of ``train_kd_and_aux`` on a batch of training nodes, with the hop feat
 
 No autograd tape: buffers are preallocated for the batch size and a step is graph-capturable (one graph per batch size).
 Dropout decisions are a pure function of (seed, step, layer, element) through the project's Philox generator.
+
+With ``gcrd=`` (a gcrd.SIGNGCRD) the step is ``train_kd_and_aux`` with ``--training nce`` (sign.py:355-367): between the
+loss and the backward the projection heads read dropout(prelu(cat)) through the same prologue, the InfoNCE runs on a sample
+of the batch, and the student head's input gradient is stored into dZcat, onto which the project FFN's first input-gradient
+GEMM accumulates; the heads' Adam follows the model's.  The step stays one CUDA graph per batch size.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 from typing import Dict, List, Optional
 
@@ -74,7 +80,9 @@ class SIGNStudentTrainer:
 
     def __init__(self, feats: List[torch.Tensor], n_classes: int, hidden: int = 512, ff_layer: int = 2, dropout: float = 0.5,
                  input_drop: float = 0.1, lr: float = 1e-3, weight_decay: float = 0, alpha: float = 0.9, kd_T: float = 4.0,
-                 batch_size: int = 50000, seed: int = 0):
+                 batch_size: int = 50000, seed: int = 0, gcrd=None):
+        """gcrd: a gcrd.SIGNGCRD built for these N nodes and the head width len(feats) * hidden; the step then adds
+        beta * G-CRD (see the module docstring) and returns [kd + beta * nce, loss_cls, nce]."""
         if weight_decay != 0:
             raise ValueError("SIGNStudentTrainer: weight_decay != 0 is not supported (sign.py's default is 0)")
         if not feats or any(not isinstance(f, torch.Tensor) or not f.is_cuda for f in feats):
@@ -91,6 +99,13 @@ class SIGNStudentTrainer:
             raise lib.B200GnnError(f"SIGNStudentTrainer: n_classes={n_classes} must be a multiple of 4, at most 512")
         if ff_layer < 1 or len(feats) > 16 or batch_size < 1 or not 0 <= dropout < 1 or not 0 <= input_drop < 1:
             raise ValueError("SIGNStudentTrainer: ff_layer >= 1, at most 16 hops, batch_size >= 1, dropout rates in [0, 1)")
+        if gcrd is not None:               # refused before any device work
+            if gcrd.H != len(feats) * hidden:
+                raise ValueError(f"gcrd=: the student head is built for width {gcrd.H}, model.out_feat is "
+                                 f"{len(feats)} hops x {hidden} = {len(feats) * hidden} wide")
+            if gcrd.N != n:
+                raise ValueError(f"gcrd=: the teacher features have {gcrd.N} rows, the hop features {n}")
+        self.gcrd = gcrd
         self.device = feats[0].device
         self.feats = list(feats)
         self.N, self.F, self.H, self.hidden, self.C, self.ff = n, F, len(feats), hidden, n_classes, ff_layer
@@ -268,7 +283,9 @@ class SIGNStudentTrainer:
                                       *self._fw(f"p.W{i}"), bias=self.P[f"p.b{i}"], out=dst)
         return a.logits[:B]
 
-    def _backward(self, B: int, d_out_feat: Optional[torch.Tensor]):
+    def _backward(self, B: int, d_out_feat: Optional[torch.Tensor], d_cat_stored: bool = False):
+        """d_out_feat: the auxiliary loss's gradient of out_feat, copied into dZcat; d_cat_stored: the G-CRD head has stored
+        it there already.  Either is the starting value of the project FFN's first input-gradient GEMM's accumulate."""
         a, H, hid, ff, p = self._tr, self.H, self.hidden, self.ff, self.p
         ops.split_tf32(self.params.view(1, -1), hi=self._split_hi.view(1, -1), lo=self._split_lo.view(1, -1))
         Zcat, dZcat = a.Zcat[:B], a.dZcat[:B]
@@ -279,7 +296,7 @@ class SIGNStudentTrainer:
             ops.col_sum_ld(G, out=self.G[f"p.b{i}"], partial=self.cs_part)
             if i == 0:
                 X, slope, bits, gslope = Zcat, self.P["slope"], a.cb(B, H * hid), self.G["slope"]
-                dst, acc, sacc = dZcat, d_out_feat is not None, False
+                dst, acc, sacc = dZcat, d_out_feat is not None or d_cat_stored, False
             else:
                 X, slope, bits, gslope = a.Zp[i - 1][:B], self._slope(None), a.hb(B, H * (ff - 1) + i - 1, hid), self._gslope(None)
                 dst, acc, sacc = a.dZp[i - 1][:B], False, i != ff - 1
@@ -300,36 +317,54 @@ class SIGNStudentTrainer:
                 ops.gemm_tf32x3_prelu_bwd(G, *self._bw(f"h{h}.W{i}"), out=a.dZh[h][i - 1][:B], z=Z, bits=bits, slope=self._slope(h),
                                           p=p, slope_grad=self._gslope(h), partial=self.slope_part, slope_accumulate=i != ff - 1)
 
-    def _check_batch(self, idx: torch.Tensor):
+    def _check_batch(self, idx: torch.Tensor, sample=None):
         if not isinstance(idx, torch.Tensor) or not idx.is_cuda or idx.dtype != torch.int64 or idx.dim() != 1:
             raise lib.B200GnnError("batch indices: expected a CUDA int64 vector")
         if not 0 < idx.numel() <= self.batch_size:
             raise ValueError(f"batch of {idx.numel()} rows: expected 1..{self.batch_size}")
+        if self.gcrd is not None:
+            self.gcrd.check_batch(idx.numel(), sample)
 
-    def _step_impl(self, idx, y, teacher_logits, aux=None, beta: float = 1.0):
+    def _check_aux(self, aux, sample=None):
+        if aux is not None and self.gcrd is not None:
+            raise ValueError("aux= and the trainer's gcrd= objective are two auxiliary losses; pass one")
+        if sample is not None and self.gcrd is None:
+            raise ValueError("sample= is the G-CRD row sample; this trainer has no gcrd= objective")
+
+    def _step_impl(self, idx, y, teacher_logits, aux=None, beta: float = 1.0, sample=None):
         B = idx.numel()
         a = self._tr
         logits = self._forward(a, idx, True, y, teacher_logits)
         ops.kd_loss_fwd_bwd(logits, a.labels[:B], None, a.teacher[:B] if teacher_logits is not None else None, self.alpha,
                             self.kd_T, d_logits=a.dlogits[:B], loss_out=self.loss_out, partial=self.kd_part)
         self._B, self._feat_stale = B, True
-        d_feat = None
-        if aux is not None:
+        d_feat, g = None, self.gcrd
+        if g is not None:
+            g.forward_backward(self, idx, a.Zcat[:B], self.P["slope"], a.cb(B, self.H * self.hidden), self.p, a.dZcat[:B],
+                               sample)
+            self.loss_out[2].copy_(g.loss_aux[0])
+        elif aux is not None:
             d_feat, self.loss_aux = aux_grad(self.out_feat(), aux, beta)
-        self._backward(B, d_feat)
+        self._backward(B, d_feat, d_cat_stored=g is not None)
         self.store.adam(self.lr)
+        if g is not None:
+            g.optimizer_step(self.lr)
         if aux is not None:
             self.loss_out[0].add_(self.loss_aux * beta)
 
     def train_step(self, batch_idx: torch.Tensor, y: torch.Tensor, teacher_logits: Optional[torch.Tensor] = None, aux=None,
-                   beta: float = 1.0) -> torch.Tensor:
+                   beta: float = 1.0, sample: Optional[torch.Tensor] = None) -> torch.Tensor:
         """One iteration of ``train_kd_and_aux`` (sign.py:293-373) on the nodes ``batch_idx`` (CUDA int64): cross-entropy
         without a teacher, kd_criterion with ``teacher_logits`` ([N, C], gathered in the step).  ``aux(out_feat)`` receives
         the batch's [B, hops*hidden] ``model.out_feat`` (requires_grad) and returns an auxiliary loss that enters as
         kd + beta*aux; heads inside it keep their gradients in the caller's autograd.  Returns the device tensor
-        [loss, loss_cls, loss_kd] (beta*aux folded into loss); no host sync."""
-        self._check_batch(batch_idx)
-        self._step_impl(batch_idx, y, teacher_logits, aux, beta)
+        [loss, loss_cls, loss_kd] (beta*aux folded into loss); no host sync.  With the trainer's gcrd= objective it returns
+        [loss + beta * nce, loss_cls, nce], and ``sample`` (positions into the batch, [S]) replaces its on-device draw."""
+        self._check_aux(aux, sample)
+        self._check_batch(batch_idx, sample)
+        if self.gcrd is not None:
+            self.gcrd.prepare([batch_idx.numel()])
+        self._step_impl(batch_idx, y, teacher_logits, aux, beta, sample)
         return self.loss_out
 
     def out_feat(self) -> torch.Tensor:
@@ -355,6 +390,13 @@ class SIGNStudentTrainer:
         """One pass of sign.py's train loop: the batches of DataLoader(train_idx, batch_size, shuffle=True,
         drop_last=False) (same sizes, every node once) in a device-drawn order.  Captured batch sizes replay their graph.
         Returns the per-step losses [n_steps, 3] (device, no sync)."""
+        self._check_aux(aux)
+        n, bs = train_idx.numel(), self.batch_size
+        sizes = [min(bs, n - s) for s in range(0, n, bs)]
+        if self.gcrd is not None:          # every batch is checked (the ragged last one too) before the first step runs
+            for B in set(sizes):
+                self.gcrd.check_batch(B)
+            self.gcrd.prepare(sizes)
         epoch = self.epoch if epoch is None else int(epoch)
         self.epoch = epoch + 1
         order = self.epoch_order(train_idx, epoch)
@@ -371,9 +413,17 @@ class SIGNStudentTrainer:
 
     def capture(self, batch_sizes, y: torch.Tensor, teacher_logits: Optional[torch.Tensor] = None):
         """Capture one CUDA graph of the step per batch size (the batch indices are read from a static buffer).  The
-        warm-up steps run on a copy of the optimiser state, which is restored: capturing does not train."""
-        with self.store.preserved():
-            for B in sorted(set(int(b) for b in batch_sizes)):
+        warm-up steps run on a copy of the optimiser state (and of the gcrd= heads' state), which is restored: capturing
+        does not train."""
+        sizes = sorted(set(int(b) for b in batch_sizes))
+        g = self.gcrd
+        if g is not None:
+            for B in sizes:
+                g.check_batch(B)
+            g.prepare(sizes)
+        heads = g.preserved() if g is not None else contextlib.nullcontext()
+        with self.store.preserved(), heads:
+            for B in sizes:
                 idx = self._idx_static[:B]
                 self._graphs[B] = capture_graph(lambda: self._step_impl(idx, y, teacher_logits), warmup=1)
         self._graph_inputs = (y, teacher_logits)
@@ -385,6 +435,8 @@ class SIGNStudentTrainer:
         self._idx_static[:B].copy_(batch_idx)
         self._graphs[B].replay()
         self._B, self._feat_stale = B, True
+        if self.gcrd is not None:
+            self.gcrd._last = self.gcrd.row_sets[B]
         return self.loss_out
 
     @torch.no_grad()

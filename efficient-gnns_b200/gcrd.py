@@ -25,6 +25,9 @@ heads and the objective are GCRD's, the row set is the graph's n nodes.
 
 ``BatchGCRD`` is the same objective for rgcn's MAG student on GraphSAINT batches, where the teacher's features and the
 number of train rows change with every batch: the row set is built per batch, on the sizes the step already holds.
+
+``SIGNGCRD`` is the same objective for engine_sign's SIGN student: every batch row is a train row, one row set per batch
+size, and the student head reads the 3072-wide dropout(prelu(cat)) through the PReLU prologue instead of a stored input.
 """
 from __future__ import annotations
 
@@ -33,7 +36,8 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import criterion, lib, ops
-from .heads import SAMPLE_STREAM, HeadRows, ProjectionHeads, _ceil4, _Pool, check_sample, check_widths  # noqa: F401
+from .heads import (SAMPLE_STREAM, HeadRows, ProjectionHeads, _ceil4, _Pool, check_sample, check_widths,  # noqa: F401
+                    draw_sample)
 
 _EPS = 1e-12                                      # F.normalize
 
@@ -263,3 +267,147 @@ class BatchGCRD(GCRD):
         hi, lo = ops.split_tf32(self.W_s, transpose=True, hi=self.WsT_split[0], lo=self.WsT_split[1])
         ops.gemm_tf32x3_rowidx(r.dz_s, hi, lo, d_feat, train_int)
         return d_feat
+
+
+class SIGNGCRD(GCRD):
+    """G-CRD inside engine_sign.SIGNStudentTrainer's captured step: the reference's ``train_kd_and_aux`` with
+    ``--training nce`` (arxiv_dgl/sign.py:355-367, heads :421-438) on every batch of B training nodes:
+
+        out_feat = student_proj(model.out_feat)          Linear(hops * hidden, proj_dim), BatchNorm1d, ReLU over all B rows
+        t_feat   = teacher_proj(teacher_out_feat[batch])  Linear(750, proj_dim), BatchNorm1d, ReLU
+        loss_aux = nce_criterion(logits, labels, out_feat, t_feat, beta, nce_T, max_samples)[2]
+        loss     = kd_criterion(logits, labels, teacher_logits, alpha, kd_T)[0] + beta * loss_aux
+        one Adam over the model and both heads
+
+    model.out_feat = dropout(prelu(cat)) is [B, hops * hidden] ([50000, 3072] at the script's settings) and is never
+    stored: the student head's Linear forms it in the A-operand prologue of ``gemm_tf32x3_prelu_stats`` from the
+    concatenation, the model slope and the keep bits, with the BatchNorm statistics in the epilogue; its weight gradient
+    is ``gemm_wgrad_tf32x3_prelu`` on the same three, transposed into gW_s.  Per step, between the trainer's loss and its
+    backward:
+
+        rows       the HeadRows of batch size B (S = min(max_samples, B)); row sets of the sizes ``prepare`` is given
+                   together are views of one _Pool (one graph per batch size, never two at once)
+        sample     only when S < B: the GCRD sampler at (trainer seed, SAMPLE_STREAM, the trainer's device step counter)
+        teacher    G_t = the zero-padded teacher features at the batch's node indices (one gather launch)
+        heads      the student front above, the teacher front, GCRD's objective, the BatchNorm backward, both weight
+                   gradients
+        d cat      dz_s . W_s stored straight into the trainer's dZcat over all B rows (every row is a train row); the
+                   project FFN's first input-gradient GEMM then accumulates onto it
+
+    Parameters, Adam state, running statistics and state-dict I/O are ProjectionHeads'."""
+
+    def __init__(self, teacher_feat: torch.Tensor, hidden: int, proj_dim: int = 256, max_samples: int = 16384,
+                 nce_T: float = 0.075, beta: float = 0.1, seed: int = 0, bn_eps: float = 1e-5, bn_momentum: float = 0.1):
+        """teacher_feat: the teacher's [N, F_t] features (the GAT teacher's ``features/`` file, F_t = 750); hidden: the
+        student head's input width, hops * hidden of the SIGN model (3072 at the script's R = 5, num_hidden = 512).  The
+        defaults are the SIGN script's (scripts/run_all_kd_and_aux.sh: beta 0.1, nce_T 0.075, max_samples 16384,
+        proj_dim 256)."""
+        if not isinstance(teacher_feat, torch.Tensor) or teacher_feat.dim() != 2 or teacher_feat.shape[0] < 1:
+            raise ValueError("teacher features must be an [N, F_t] tensor")
+        hidden = int(hidden)
+        if int(max_samples) < 1:
+            raise ValueError("max_samples must be at least 1")
+        if not ops.gemm_stats_supported(proj_dim):
+            raise ValueError("proj_dim must be a multiple of 32 in (48, 256]")
+        if hidden % 32 or hidden <= 0:
+            raise ValueError("the student head's width (hops * hidden) must be a positive multiple of 32")
+        if not 0 < _ceil4(teacher_feat.shape[1]) <= 2048:
+            raise ValueError("teacher feature width must be at most 2048 (the teacher head's weight-gradient GEMM)")
+        self._init_heads(hidden, proj_dim, int(teacher_feat.shape[1]), beta, seed, bn_eps, bn_momentum, teacher_feat.device)
+        self.nce_T, self.max_samples = float(nce_T), int(max_samples)
+        self.N = int(teacher_feat.shape[0])
+        # every row's teacher features at a 16-byte pitch; the padding columns must be zeros (W_t's zero columns do not
+        # cancel a NaN)
+        self.t_feat = torch.zeros(self.N, self.Ft_pad, device=self.device)
+        self.t_feat[:, :self.F_t].copy_(teacher_feat.detach().to(torch.float32))
+        H, P = self.H, self.P
+        # the student head's weight gradient [H, P], column blocks of WGRAD_PRELU_BLOCK when H > 2048, then transposed
+        self.gWs_T = torch.empty(H, P, device=self.device)
+        self.wgrad_ws_s = torch.empty(ops.wgrad_workspace_floats(H if H <= 2048 else ops.WGRAD_PRELU_BLOCK, P),
+                                      device=self.device)
+        self.row_sets = {}                                  # batch size -> HeadRows
+        self._pools = []                                  # keeps every pool's buffers alive (captured graphs read them)
+        self._last: Optional[HeadRows] = None
+
+    def prepare(self, batch_sizes: Sequence[int]):
+        """Build the row sets of these batch sizes (those not built yet) on one _Pool: one buffer per request, sized for the
+        largest; the operands' padding rows stay zero (every size's S rows end at row S_max of one zeroed buffer)."""
+        new = sorted({int(b) for b in batch_sizes} - set(self.row_sets))
+        if not new:
+            return
+        dev, P, Ftp = self.device, self.P, self.Ft_pad
+        samples = [min(self.max_samples, B) for B in new]
+        S_max = max(samples)
+        flat_s, flat_t = (torch.zeros((S_max + 3) * P, device=dev) for _ in range(2))
+
+        def operands(S):
+            o, Sp = (S_max - S) * P, _ceil4(S)
+            return flat_s[o:o + Sp * P].view(Sp, P), flat_t[o:o + Sp * P].view(Sp, P)
+
+        def build(B, S, alloc):
+            G_t = alloc(B, Ftp)
+            return HeadRows(self, B, S, G_t, *operands(S), alloc)
+
+        pool = _Pool(dev)
+        for B, S in zip(new, samples):
+            build(B, S, pool.recorder())
+        n_draw = max((B for B, S in zip(new, samples) if S < B), default=0)
+        ws = (torch.empty(int(lib.load().b200gnn_gcrd_sample_workspace_bytes(n_draw)), dtype=torch.uint8, device=dev)
+              if n_draw else None)
+        for B, S in zip(new, samples):
+            r = build(B, S, pool.views())
+            r.sample_ws = ws
+            self.row_sets[B] = r
+        self._pools.append((pool, flat_s, flat_t, ws))
+
+    def check_batch(self, B: int, sample=None):
+        """ValueError for a batch the step cannot take (one row: BatchNorm has no variance, as the reference's BatchNorm1d
+        raises), or a sample that is not S = min(max_samples, B) distinct positions in [0, B)."""
+        if B == 1:
+            raise ValueError("a batch of one row: the projection heads' BatchNorm needs more than one value per channel "
+                             "in training")
+        if sample is not None:
+            check_sample(sample, B, min(self.max_samples, B))
+
+    @property
+    def loss_aux(self) -> torch.Tensor:
+        return self._last.loss_aux if self._last is not None else torch.full((1,), float("nan"), device=self.device)
+
+    def sample(self) -> torch.Tensor:
+        """The last step's sample: positions into its batch (int64 [S])."""
+        return self._last.inds.to(torch.int64)
+
+    def _draw(self, tr, r: HeadRows, sample: Optional[torch.Tensor]):
+        draw_sample(tr, r.n, r.S, r.perm, r.sample_ws, sample)
+
+    def _front_student(self, r: HeadRows, src):
+        Z, slope, bits, p = src
+        hi, lo = ops.split_tf32(self.W_s, hi=self.Ws_split[0], lo=self.Ws_split[1])
+        ops.gemm_tf32x3_prelu_stats(Z, slope, bits, p, hi, lo, self.b_s, r.pre_s, r.gp_s)
+        ops.bn_finalize(r.gp_s, r.n, self.gamma_s, self.beta_s, self.bn_eps, self.bn_momentum, self.rm_s, self.rv_s,
+                        out=self.bn_s)
+
+    def _wgrad_student(self, r: HeadRows, src):
+        Z, slope, bits, p = src
+        ops.gemm_wgrad_tf32x3_prelu(Z, slope, bits, p, r.dz_s, out=self.gWs_T, workspace=self.wgrad_ws_s)
+        lib.check(lib.load().b200gnn_transpose_f32(lib.dptr(self.gWs_T, torch.float32, "gWs_T"), self.H, self.P,
+                                                   lib.dptr(self.gW_s, torch.float32, "gW_s"), lib.stream_ptr()),
+                  "transpose_f32")
+
+    def forward_backward(self, tr, idx: torch.Tensor, zcat: torch.Tensor, slope: torch.Tensor, bits: torch.Tensor, p: float,
+                         d_zcat: torch.Tensor, sample: Optional[torch.Tensor] = None):
+        """The objective of the batch ``idx`` (int64 [B] node indices; its row set must have been prepared): reads
+        out_feat = dropout(prelu(zcat)) through (zcat [B, H], slope, bits [B, H/32], p), STORES d (beta * loss_aux) /
+        d out_feat into d_zcat [B, H] and adds beta * loss_aux to tr.loss_out[0].  Enqueues launches only (capturable)
+        unless ``sample`` (positions into the batch, [S]) replaces the draw."""
+        B = idx.numel()
+        r = self.row_sets[B]
+        self._last = r
+        self._draw(tr, r, sample)
+        ops.gather_rows_act(self.t_feat, idx, r.G_t)
+        src = (zcat, slope, bits, p)
+        self._front(r, src)
+        self._objective(tr, r)
+        self._tail(r, src)
+        hi, lo = ops.split_tf32(self.W_s, transpose=True, hi=self.WsT_split[0], lo=self.WsT_split[1])
+        ops.gemm_tf32x3(r.dz_s, hi, lo, out=d_zcat)

@@ -22,7 +22,9 @@ buffers (``_Pool``).  Its ``forward_backward`` runs, as launches only (capturabl
                  rows of d out_feat
 
 The draw, the heads, the objective and the tail (``_draw``, ``_front``, ``_objective``, ``_tail``) take the row set, so the
-per-graph form runs the same launches with no gather and its own store of the input gradient.
+per-graph form runs the same launches with no gather and its own store of the input gradient.  The student head's halves
+of the front and the tail (``_front_student``, ``_wgrad_student``) are separate, so gcrd.SIGNGCRD, whose head reads the
+un-stored dropout(prelu(cat)), replaces them alone.
     Adam         over the heads' flat buffer, after the trainer's own Adam (same lr: one Adam over three groups)
 
 The sample cannot equal numpy's ``np.random.choice`` draw; ``train_step(..., sample=)`` injects one (tests).
@@ -282,30 +284,45 @@ class ProjectionHeads:
         """The step's sample into r.perm: the injected one, or the on-device draw when S < n (none when S = n)."""
         draw_sample(tr, r.n, r.S, r.perm, self.sample_ws, sample)
 
-    def _front(self, r: HeadRows, G_s: torch.Tensor):
+    def _front(self, r: HeadRows, G_s):
         """Both heads' Linear over the row set with the BatchNorm statistics in the GEMM epilogue, then finalize (running
-        statistics).  G_s: the student head's input [n, H]."""
-        for G, W, b, gamma, beta, rm, rv, pre, gp, bn, split in (
-                (G_s, self.W_s, self.b_s, self.gamma_s, self.beta_s, self.rm_s, self.rv_s, r.pre_s, r.gp_s, self.bn_s,
-                 self.Ws_split),
-                (r.G_t, self.W_t, self.b_t, self.gamma_t, self.beta_t, self.rm_t, self.rv_t, r.pre_t, r.gp_t, self.bn_t,
-                 self.Wt_split)):
-            hi, lo = ops.split_tf32(W, hi=split[0], lo=split[1])
-            ops.gemm_tf32x3_stats(G, hi, lo, b, pre, gp)
-            ops.bn_finalize(gp, r.n, gamma, beta, self.bn_eps, self.bn_momentum, rm, rv, out=bn)
+        statistics).  G_s: the student head's input, as ``_front_student`` reads it."""
+        self._front_student(r, G_s)
+        self._front_teacher(r)
 
-    def _tail(self, r: HeadRows, G_s: torch.Tensor):
+    def _front_student(self, r: HeadRows, G_s):
+        """The student half of ``_front``; G_s the head's input [n, H].  A subclass whose student head reads its input in
+        another form overrides this and ``_wgrad_student``."""
+        hi, lo = ops.split_tf32(self.W_s, hi=self.Ws_split[0], lo=self.Ws_split[1])
+        ops.gemm_tf32x3_stats(G_s, hi, lo, self.b_s, r.pre_s, r.gp_s)
+        ops.bn_finalize(r.gp_s, r.n, self.gamma_s, self.beta_s, self.bn_eps, self.bn_momentum, self.rm_s, self.rv_s,
+                        out=self.bn_s)
+
+    def _front_teacher(self, r: HeadRows):
+        hi, lo = ops.split_tf32(self.W_t, hi=self.Wt_split[0], lo=self.Wt_split[1])
+        ops.gemm_tf32x3_stats(r.G_t, hi, lo, self.b_t, r.pre_t, r.gp_t)
+        ops.bn_finalize(r.gp_t, r.n, self.gamma_t, self.beta_t, self.bn_eps, self.bn_momentum, self.rm_t, self.rv_t,
+                        out=self.bn_t)
+
+    def _tail(self, r: HeadRows, G_s):
         """The BatchNorm backward apply over the row set and both heads' weight gradients; the student head's input
         gradient r.dz_s . W_s is the caller's."""
-        L, st = lib.load(), lib.stream_ptr()
         for dz, pre, bn, gamma, part, gg, gbe, gb in (
                 (r.dz_s, r.pre_s, self.bn_s, self.gamma_s, self.bpart_s, self.ggamma_s, self.gbeta_s, self.gb_s),
                 (r.dz_t, r.pre_t, self.bn_t, self.gamma_t, self.bpart_t, self.ggamma_t, self.gbeta_t, self.gb_t)):
             ops.bn_act_bwd_apply(dz, None, pre, bn[0], bn[1], gamma, part, r.n, 0.0, dz, gg, gbe, gb, r.rows_part, self.coef)
+        self._wgrad_student(r, G_s)
+        self._wgrad_teacher(r)
+
+    def _wgrad_student(self, r: HeadRows, G_s):
+        """gW_s = r.dz_s^T . G_s: the student half of ``_tail``."""
         ops.gemm_wgrad_tf32x3(r.dz_s, G_s, out=self.gW_s, workspace=self.wgrad_ws, wide=self.ws_wide)
+
+    def _wgrad_teacher(self, r: HeadRows):
         ops.gemm_wgrad_tf32x3(r.G_t, r.dz_t, out=self.gWt_T, workspace=self.wgrad_ws, wide=True)
-        lib.check(L.b200gnn_transpose_f32(lib.dptr(self.gWt_T, torch.float32, "gWt_T"), self.Ft_pad, self.P,
-                                          lib.dptr(self.gW_t, torch.float32, "gW_t"), st), "transpose_f32")
+        lib.check(lib.load().b200gnn_transpose_f32(lib.dptr(self.gWt_T, torch.float32, "gWt_T"), self.Ft_pad, self.P,
+                                                   lib.dptr(self.gW_t, torch.float32, "gW_t"), lib.stream_ptr()),
+                  "transpose_f32")
 
     def _objective(self, tr, r: HeadRows):
         """The objective between the head front and the tail on row set r (see the module docstring); enqueues launches

@@ -113,6 +113,8 @@ SIGNATURES = {
                                                  _f32p, _ptr]),
     "b200gnn_gemm_tf32x3_prelu_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p,
                                              _f32p, _ptr, _f32, _ptr]),
+    "b200gnn_gemm_tf32x3_prelu_stats_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _f32p,
+                                                   _f32p, _ptr, _f32, _f32p, _i64, _ptr]),
     "b200gnn_gemm_tf32x3_prelu_bwd_f32": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _f32p, _i64, _i64, _i64, _i64, _int,
                                                  _f32p, _ptr, _f32p, _f32, _f32p, _int, _ptr, _i64, _ptr]),
     "b200gnn_gemm_wgrad_tf32x3_prelu_f32": (_int, [_f32p, _i64, _f32p, _i64, _f32p, _i64, _i64, _i64, _f32p, _ptr, _i64, _f32,

@@ -768,6 +768,26 @@ def gemm_tf32x3_prelu(z: torch.Tensor, slope: torch.Tensor, bits: torch.Tensor, 
     return out
 
 
+def gemm_tf32x3_prelu_stats(z: torch.Tensor, slope: torch.Tensor, bits: torch.Tensor, p: float, b_hi: torch.Tensor,
+                            b_lo: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor,
+                            partial: torch.Tensor) -> torch.Tensor:
+    """out = dropout(prelu(z)) @ b^T + bias with the BatchNorm batch statistics of ``out`` in the epilogue: output and
+    partial[slots, 2, N] bit for bit ``gemm_tf32x3_stats`` of ``prelu_bits(z, bits, slope, p)``, the activation never
+    materialised.  N a multiple of 32 in (48, 256]."""
+    M, K = z.shape
+    N = b_hi.shape[0]
+    assert b_hi.shape == b_lo.shape and b_hi.shape[1] == K
+    zp, lda = _rows(z, "z")
+    if bits.shape[1] != (K + 31) // 32:
+        raise lib.B200GnnError("gemm_tf32x3_prelu_stats: keep bits must be [M, ceil(K/32)]")
+    lib.check(lib.load().b200gnn_gemm_tf32x3_prelu_stats_f32(zp, lda, _f32(b_hi, "b_hi"), _f32(b_lo, "b_lo"), b_hi.stride(0),
+                                                             _f32(out, "out"), out.stride(0), M, N, K, _f32(bias, "bias"),
+                                                             _f32(slope, "slope"), _bits(bits, M, K), float(p),
+                                                             _f32(partial, "partial"), partial.shape[0], lib.stream_ptr()),
+              "gemm_tf32x3_prelu_stats_f32")
+    return out
+
+
 def gemm_tf32x3_prelu_bwd(a: torch.Tensor, b_hi: torch.Tensor, b_lo: torch.Tensor, out: torch.Tensor, z: torch.Tensor,
                           bits: torch.Tensor, slope: torch.Tensor, p: float, slope_grad: torch.Tensor, partial: torch.Tensor,
                           accumulate: bool = False, slope_accumulate: bool = False) -> torch.Tensor:

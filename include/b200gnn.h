@@ -414,6 +414,9 @@ int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, const float* 
  * b200gnn_dropout_bits_u32 (bit c % 32 of word c / 32 of a row).
  *   _gemm_tf32x3_prelu_f32      : C = x · B^T (+ bias), x formed from Z in the GEMM's registers (bits uint32 [M][ceil(K/32)]),
  *                                 bit for bit the product of the activation b200gnn_prelu_bits_f32 materialises.  Any K.
+ *   _gemm_tf32x3_prelu_stats_f32: _gemm_tf32x3_prelu_f32 with the BatchNorm batch statistics of C in the epilogue: output and
+ *                                 partial[slots][2][N] bit for bit those of _gemm_tf32x3_stats_f32 on that activation (same
+ *                                 refusals: N a multiple of 32 in (48, 256], C 16-byte aligned, ldc % 4 == 0).
  *   _gemm_tf32x3_prelu_bwd_f32  : the input-gradient GEMM behind x: dA = A · B^T (+ C if accumulate); what is STORED to C is
  *                                 dZ = (bit ? dA/(1-p) : 0) * (Z > 0 ? 1 : slope) (Z: [M, ldc] like C, bits [M][N/32], N a
  *                                 multiple of 32); slope_grad = (slope_accumulate ? slope_grad : 0) + sum over Z <= 0 of
@@ -433,6 +436,10 @@ int b200gnn_gemm_wgrad_tf32x3_act_f32(const float* Y, int64_t ldx, const float* 
 int b200gnn_gemm_tf32x3_prelu_f32(const float* Z, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
                                   float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
                                   const float* slope, const uint32_t* bits, float p_drop, void* stream);
+int b200gnn_gemm_tf32x3_prelu_stats_f32(const float* Z, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
+                                        float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias,
+                                        const float* slope, const uint32_t* bits, float p_drop, float* partial, int64_t slots,
+                                        void* stream);
 int b200gnn_gemm_tf32x3_prelu_bwd_f32(const float* A, int64_t lda, const float* B_hi, const float* B_lo, int64_t ldb,
                                       float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, int accumulate,
                                       const float* Z, const uint32_t* bits, const float* slope, float p_drop,
